@@ -127,6 +127,54 @@ YB_API int yb_box_iou(const float* a, int n, const float* b, int m, float* out, 
 YB_API int yb_mask_rle(const uint32_t* bits, int n, int h, int w, uint32_t* counts, int max_runs, int32_t* nruns, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Evaluation: box and mask mAP -- replaces utils/common_utils.py:107-255 (APDataObject, prep_metrics, calc_map) as eval.py:35-69
+ * and :106 drive them, batched over images.  Results equal the reference's float64 values bit for bit:
+ *   yb_eval_match  per image: box IoU (scaled gt vs int pixel boxes, fp32) and popcount mask IoU for same-class pairs, then
+ *                  prep_metrics' greedy matching for every (IoU type, threshold): detections of a class in their given order,
+ *                  each takes the unused gt of its class with the largest IoU > thr (compared in double; ties -> earliest gt;
+ *                  NaN never matches).  Appends one record (score, class, tp bits) per detection at the image's position in
+ *                  the caller's record buffers (running count + exclusive prefix of earlier images' counts: no host sync) and
+ *                  adds the image's per-class gt counts and "seen" flags.  Images with count == 0 contribute nothing
+ *                  (eval.py:53 skips them before prep_metrics, so their gts are never counted).
+ *                  tp bit (type * num_thr + t): type 0 = box, 1 = mask.
+ *  yb_eval_ap      APDataObject.get_ap for every (type, threshold, class): stable sort of the records by (class, descending
+ *                  score; ties keep record order = image order, then detection order), precision / recall in double, the
+ *                  running max from the right, np.searchsorted(recalls, x / 100, 'left') at 101 points, their sum in order with
+ *                  the Neumaier compensation of Python's sum() (CPython >= 3.12) / 101;
+ *                  0 when the class has no gt.  ap [2][num_thr][num_classes] float64, nonempty [num_classes] (1 iff the class
+ *                  occurred among the detections or gts of an evaluated image: !APDataObject.is_empty()).
+ * Inputs of yb_eval_match (DEVICE pointers; batch B, max_det D):
+ *   count [B], cls [B,D] (0-based class), score [B,D]: detect_batched's record layout; box_px [B,D,4] int32 pixel boxes (after_nms)
+ *   det_masks: packed masks (yb_pack_mask_bits layout) of all images back to back; image b owns words det_mask_off[b] ..
+ *              det_mask_off[b+1] (int64 [B+1]), at least count[b] masks of img_hw[b] = (h, w) (int32 [B,2]); det_mask_words =
+ *              words in det_masks
+ *   gt [total_gt,5] (x1,y1,x2,y2 in [0,1], class) and gt_offset [B+1] as in yb_losses; gt_masks / gt_mask_off / gt_mask_words
+ *              likewise for the packed gt masks, exactly one per gt row (gt row r of image b is mask r - gt_offset[b] of the image)
+ *   records: rec_score / rec_cls / rec_tp [capacity]; classes outside [0, num_classes) are stored as -1 and never counted
+ *   state [yb_eval_state_bytes]: zeroed by the caller before the first batch.  Bytes 0-7: records appended so far (uint64);
+ *              bytes 12-15: error flags (bit 0: capacity exceeded, bit 1: an image's gt or mask ranges lie outside the buffers
+ *              or do not match its geometry; such an image's records are stored with class -1).
+ * ---------------------------------------------------------------------------------------- */
+#define YB_EVAL_MAX_THR 16
+typedef struct {
+  int num_classes;                 /* len(cfg.class_names) */
+  int num_thr;                     /* len(iou_thres), 1 .. YB_EVAL_MAX_THR (eval.py uses 10) */
+  double thr[YB_EVAL_MAX_THR];     /* iou_thres (eval.py:24): x / 100 */
+} yb_eval_params;
+
+YB_API size_t yb_eval_state_bytes(const yb_eval_params* p);
+YB_API size_t yb_eval_match_workspace_bytes(int batch, int max_det, int64_t total_gt, const yb_eval_params* p);
+YB_API size_t yb_eval_ap_workspace_bytes(int64_t num_records, const yb_eval_params* p);
+YB_API int yb_eval_match(const yb_eval_params* p, int batch, int max_det, const int32_t* count, const int32_t* cls, const float* score,
+                         const int32_t* box_px, const uint32_t* det_masks, const int64_t* det_mask_off, int64_t det_mask_words,
+                         const int32_t* img_hw, const float* gt, const int32_t* gt_offset, int64_t total_gt, const uint32_t* gt_masks,
+                         const int64_t* gt_mask_off, int64_t gt_mask_words, float* rec_score, int32_t* rec_cls, uint32_t* rec_tp,
+                         int64_t capacity, void* state, void* workspace, size_t workspace_bytes, void* stream);
+/* num_records: an upper bound of the records appended (the records beyond the state's count are ignored) */
+YB_API int yb_eval_ap(const yb_eval_params* p, const float* rec_score, const int32_t* rec_cls, const uint32_t* rec_tp, int64_t num_records,
+                      const void* state, void* workspace, size_t workspace_bytes, double* ap, uint8_t* nonempty, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Pre-process -- replaces utils/augmentations.py:219-227 val_aug(img, val_size) (SURVEY.md 8(f) #1):
  * uint8 BGR HWC image [h,w,3] (device) -> float32 RGB CHW [3,S,S] (device): pad to square at the
  * top-left with the BGR mean, bilinear resize (OpenCV INTER_LINEAR coordinates), (x-mean)/std.

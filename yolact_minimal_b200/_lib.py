@@ -37,6 +37,13 @@ class LossParams(C.Structure):
                 ('mask_alpha', C.c_float), ('semantic_alpha', C.c_float)]
 
 
+EVAL_MAX_THR = 16
+
+
+class EvalParams(C.Structure):
+    _fields_ = [('num_classes', C.c_int), ('num_thr', C.c_int), ('thr', C.c_double * EVAL_MAX_THR)]
+
+
 class TrainHparams(C.Structure):
     _fields_ = [('pos_iou_thr', C.c_float), ('neg_iou_thr', C.c_float), ('neg_pos_ratio', C.c_int), ('masks_to_train', C.c_int),
                 ('conf_alpha', C.c_float), ('bbox_alpha', C.c_float), ('mask_alpha', C.c_float), ('semantic_alpha', C.c_float),
@@ -64,6 +71,12 @@ PROTOTYPES = {
     'yb_mask_iou_bits': (C.c_int, [vp, C.c_int, vp, C.c_int, C.c_int64, vp, vp]),
     'yb_box_iou': (C.c_int, [vp, C.c_int, vp, C.c_int, vp, vp]),
     'yb_mask_rle': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp]),
+    'yb_eval_state_bytes': (C.c_size_t, [C.POINTER(EvalParams)]),
+    'yb_eval_match_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.POINTER(EvalParams)]),
+    'yb_eval_ap_workspace_bytes': (C.c_size_t, [C.c_int64, C.POINTER(EvalParams)]),
+    'yb_eval_match': (C.c_int, [C.POINTER(EvalParams), C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp, C.c_int64,
+                                vp, vp, C.c_int64, vp, vp, vp, C.c_int64, vp, vp, C.c_size_t, vp]),
+    'yb_eval_ap': (C.c_int, [C.POINTER(EvalParams), vp, vp, vp, C.c_int64, vp, vp, C.c_size_t, vp, vp, vp]),
     'yb_net_create': (C.c_int, [C.POINTER(NetConfig), C.POINTER(vp)]),
     'yb_net_destroy': (None, [vp]),
     'yb_net_num_params': (C.c_int, [vp]),

@@ -7,6 +7,7 @@
 //                           column-major runs starting with a run of zeros; the ASCII compression of the counts is host work
 // All HBM-bound streaming kernels: every packed word is read once per use.
 #include "common.cuh"
+#include "iou.cuh"
 
 #include <stdint.h>
 
@@ -32,8 +33,7 @@ __global__ void __launch_bounds__(256) k_mask_iou_bits(const uint32_t* __restric
   const uint32_t* pb = b + (size_t)j * words;
   unsigned inter = 0, ca = 0, cb = 0;
   for (long long k = threadIdx.x; k < words; k += 256) {
-    const uint32_t x = pa[k], y = pb[k];
-    inter += __popc(x & y); ca += __popc(x); cb += __popc(y);
+    mask_counts_add(pa[k], pb[k], inter, ca, cb);
   }
   __shared__ unsigned s[3][256];
   s[0][threadIdx.x] = inter; s[1][threadIdx.x] = ca; s[2][threadIdx.x] = cb;
@@ -42,10 +42,7 @@ __global__ void __launch_bounds__(256) k_mask_iou_bits(const uint32_t* __restric
     if (threadIdx.x < off) { s[0][threadIdx.x] += s[0][threadIdx.x + off]; s[1][threadIdx.x] += s[1][threadIdx.x + off]; s[2][threadIdx.x] += s[2][threadIdx.x + off]; }
     __syncthreads();
   }
-  if (threadIdx.x == 0) {
-    const float fi = (float)s[0][0];
-    out[(size_t)i * m + j] = __fdiv_rn(fi, __fsub_rn(__fadd_rn((float)s[1][0], (float)s[2][0]), fi));
-  }
+  if (threadIdx.x == 0) out[(size_t)i * m + j] = mask_iou_from_counts(s[0][0], s[1][0], s[2][0]);
 }
 
 // ---- pairwise box IoU (utils/box_utils.py:8-37, separately rounded operations) ----
@@ -53,13 +50,7 @@ __global__ void k_box_iou(const float* __restrict__ a, int n, const float* __res
   const int t = blockIdx.x * 256 + threadIdx.x;
   if (t >= n * m) return;
   const int i = t / m, j = t - i * m;
-  const float4 p = reinterpret_cast<const float4*>(a)[i], q = reinterpret_cast<const float4*>(b)[j];
-  const float iw = fmaxf(__fsub_rn(fminf(p.z, q.z), fmaxf(p.x, q.x)), 0.f);
-  const float ih = fmaxf(__fsub_rn(fminf(p.w, q.w), fmaxf(p.y, q.y)), 0.f);
-  const float inter = __fmul_rn(iw, ih);
-  const float aa = __fmul_rn(__fsub_rn(p.z, p.x), __fsub_rn(p.w, p.y));
-  const float ab = __fmul_rn(__fsub_rn(q.z, q.x), __fsub_rn(q.w, q.y));
-  out[t] = __fdiv_rn(inter, __fsub_rn(__fadd_rn(aa, ab), inter));
+  out[t] = box_iou_rn(reinterpret_cast<const float4*>(a)[i], reinterpret_cast<const float4*>(b)[j]);
 }
 
 // ---- COCO run-length encoding of packed masks: column-major scan (x outer, y inner), first run counts zeros ----
