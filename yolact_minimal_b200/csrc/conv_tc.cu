@@ -394,17 +394,24 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 }
 
 // =================================================================================================================
-// Fused bottleneck tail + next head (layers.cuh BneckArgs), one CTA per 128-row tile, the same three warpgroups:
+// Fused bottleneck tail + next head (layers.cuh BneckArgs), persistent, one 128-row tile at a time, the same three warpgroups:
 //   for each 128-channel chunk c of the expanded width:
 //     A(c):  accA  = t2 * W3_c^T                 (wgmma m64n128, K = Cmid [+ Cd: the folded downsample branch])
-//     E(c):  x'_c  = relu(accA + b3_c [+ x_c])   -> 16 bit -> xo in HBM, and into shared memory in the 128B-swizzled A-operand layout
+//     E(c):  x'_c  = relu(accA + b3_c [+ x_c])   -> 16 bit, in shared memory in the 128B-swizzled A-operand layout -> xo (TMA store)
 //     B(c):  accB += x'_c * W1_c^T               (wgmma m64nCmid, K = 128)
 //   t1 = relu(accB + b1) -> HBM.
 // x' never makes a round trip through HBM before the next block's conv1.  The operand rounding points, the k order and the epilogue
 // arithmetic are those of the two separate k_conv_tc launches, so the result is bit-identical to the unfused pair (the folded
-// downsample branch skips one 16-bit rounding of the residual).  The t2 tile stays resident for the whole tile; the W3 / W1 k-blocks
-// stream through a ring in exactly the order the consumers use them.  Both GEMMs' accumulators live in registers (64 + Cmid / 2 per
+// downsample branch skips one 16-bit rounding of the residual).  Both GEMMs' accumulators live in registers (64 + Cmid / 2 per
 // thread), so the consumers take 232 registers from the producer with setmaxnreg.
+//
+// Shared memory: the t2 tile (resident for the whole tile), two x buffers and a ring of weight slots in the order the consumers use
+// them.  An x buffer is one chunk, [2 k-blocks][128 rows x 128 B] in the A-operand layout.  The producer loads the residual chunk x_c
+// into it by TMA one chunk ahead; E(c) reads x_c and writes x'_c at the same swizzled address, so the buffer is in turn the residual,
+// the A operand of B(c) and the source of the TMA store of xo (rows >= M are clipped by the store's tensor map).  A buffer is handed
+// back to the producer once B(c) has retired and the store has read it.  Both GEMMs keep one k-block in flight and release a slot
+// when it retires; B(c)'s last k-block retires under A(c+1).  At Cmid = 256 one 32 KiB slot holds either two W3 k-blocks or one
+// W1 k-block.
 // =================================================================================================================
 struct BnParams {
   long long M;
@@ -413,31 +420,45 @@ struct BnParams {
   Geom g;
   const float* b3;
   const float* b1;
-  const void* x;
-  void* xo;
   void* t1;
 };
 
 __device__ __forceinline__ void named_barrier_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ uint32_t lds32(uint32_t a) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
+__device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+
+constexpr uint32_t BN_X_BYTES = 2 * TC_A_STAGE;                  // one x buffer: 128 rows x 128 channels
 
 template <bool F16, int CMID>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUtensorMap tmXd, const __grid_constant__ CUtensorMap tmW3,
-           const __grid_constant__ CUtensorMap tmW1, const BnParams p) {
+           const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXo,
+           const BnParams p) {
+  constexpr int WPS = CMID == 256 ? 2 : 1;                       // W3 k-blocks per ring slot
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* sT2 = smem;                                         // [kbA][128 rows x 128 B]
-  uint8_t* sX = sT2 + (size_t)p.kbA * TC_A_STAGE;              // [2 warpgroups][2 k-blocks][64 rows x 128 B]
-  uint8_t* sRing = sX + 2 * TC_A_STAGE;                        // [slots][slot_bytes]
+  uint8_t* sX = sT2 + (size_t)p.kbA * TC_A_STAGE;              // [2 buffers][2 k-blocks][128 rows x 128 B]
+  uint8_t* sRing = sX + 2 * BN_X_BYTES;                        // [slots][slot_bytes]
   uint64_t* full = reinterpret_cast<uint64_t*>(sRing + (size_t)p.slots * p.slot_bytes);
   uint64_t* empty = full + TC_MAX_STAGES;
   uint64_t* t2_full = empty + TC_MAX_STAGES;
   uint64_t* t2_empty = t2_full + 1;
+  uint64_t* x_full = t2_empty + 1;                             // [2]
+  uint64_t* x_empty = x_full + 2;                              // [2]
 
   const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
     for (int i = 0; i < TC_MAX_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], 8); }
     mbar_init(t2_full, 1); mbar_init(t2_empty, 8);
+    for (int i = 0; i < 2; ++i) { mbar_init(&x_full[i], 1); mbar_init(&x_empty[i], 8); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -449,17 +470,29 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
     if (threadIdx.x == 0) {
       griddep_wait();
       int stage = 0; uint32_t phase = 0;
+      int q = 0;                                                 // chunk count over all tiles: x buffer q & 1
       for (int i = 0, tile = (int)blockIdx.x; tile < p.m_tiles; ++i, tile += (int)gridDim.x) {
         const int row0 = tile * TC_BM;
         mbar_wait(t2_empty, (uint32_t)(i & 1) ^ 1u);                // the previous tile's A GEMMs have read the resident t2 tile
         mbar_expect_tx(t2_full, (uint32_t)p.kbA * TC_A_STAGE);
         for (int kb = 0; kb < p.kbA; ++kb)                          // t2's k-blocks, then the block input's (folded downsample)
           tma_load_2d(sT2 + (size_t)kb * TC_A_STAGE, kb < p.kbT ? &tmT2 : &tmXd, (kb < p.kbT ? kb : kb - p.kbT) * TC_BK, row0, t2_full);
-        for (int c = 0; c < p.nch; ++c) {
-          for (int kb = 0; kb < p.kbA; ++kb) {                      // W3 rows c*128 .., k-block kb
+        for (int c = 0; c < p.nch; ++c, ++q) {
+          const int xb = q & 1;
+          mbar_wait(&x_empty[xb], (uint32_t)((q >> 1) & 1) ^ 1u);   // B(q-2) has retired and xo's store has read the buffer
+          if (p.has_res) {
+            mbar_expect_tx(&x_full[xb], BN_X_BYTES);
+            for (int kb = 0; kb < 2; ++kb)
+              tma_load_2d(sX + (size_t)xb * BN_X_BYTES + (size_t)kb * TC_A_STAGE, &tmX, c * 128 + kb * TC_BK, row0, &x_full[xb]);
+          } else {
+            mbar_arrive(&x_full[xb]);                               // folded branch: no residual, the buffer only holds x'
+          }
+          for (int kb = 0; kb < p.kbA; kb += WPS) {                 // W3 rows c*128 .., k-blocks kb .. kb + WPS - 1
             mbar_wait(&empty[stage], phase ^ 1);
-            mbar_expect_tx(&full[stage], TC_A_STAGE);
-            tma_load_2d(sRing + (size_t)stage * p.slot_bytes, &tmW3, kb * TC_BK, c * 128, &full[stage]);
+            mbar_expect_tx(&full[stage], WPS * TC_A_STAGE);
+#pragma unroll
+            for (int w = 0; w < WPS; ++w)
+              tma_load_2d(sRing + (size_t)stage * p.slot_bytes + (size_t)w * TC_A_STAGE, &tmW3, (kb + w) * TC_BK, c * 128, &full[stage]);
             if (++stage == p.slots) { stage = 0; phase ^= 1; }
           }
           for (int kb = 0; kb < 2; ++kb) {                          // W1[:, c*128 + kb*64 ..]: all CMID rows
@@ -478,10 +511,17 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
     const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
     const bool signal = lane == 0;
     griddep_wait();
-    uint8_t* sXw = sX + (size_t)cw * TC_A_STAGE;                   // this warpgroup's x' chunk: two k-blocks of [64 rows x 128 B]
     float accA[64];
     float accB[CMID / 2];
     int stage = 0; uint32_t phase = 0;
+    int prev = -1;                                               // ring slot whose MMAs are still in flight
+    int xpend = -1;                                              // x buffer read by the in-flight B(c)
+    auto release = [&](int s) { if (signal) mbar_arrive(&empty[s]); };
+    auto release_x = [&](int b) {                                // B(c) has retired: hand the buffer back once xo's store has read it
+      if (t == 0) bulk_wait_read0();
+      if (signal) mbar_arrive(&x_empty[b]);
+    };
+    int q = 0;
     for (int i = 0, tile = (int)blockIdx.x; tile < p.m_tiles; ++i, tile += (int)gridDim.x) {
       long long m[2];
       bool valid[2], zero[2];
@@ -497,51 +537,69 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
         }
       }
       mbar_wait(t2_full, (uint32_t)(i & 1));
-      for (int c = 0; c < p.nch; ++c) {
+      for (int c = 0; c < p.nch; ++c, ++q) {
+        const int xb = q & 1;
         // ---- A(c) ----
-        for (int kb = 0; kb < p.kbA; ++kb) {
+        for (int kb = 0; kb < p.kbA; kb += WPS) {
           mbar_wait(&full[stage], phase);
-          const uint64_t da = gmma_desc(smem_u32(sT2 + (size_t)kb * TC_A_STAGE + (size_t)cw * (TC_A_STAGE / 2)));
-          const uint64_t db = gmma_desc(smem_u32(sRing + (size_t)stage * p.slot_bytes));
+          const uint32_t slot = smem_u32(sRing + (size_t)stage * p.slot_bytes);
           acc_fence<64>(accA);
           wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k) wgmma_n128<F16, 0>(accA, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) != 0 ? 1u : 0u);
+          for (int w = 0; w < WPS; ++w) {
+            const uint64_t da = gmma_desc(smem_u32(sT2 + (size_t)(kb + w) * TC_A_STAGE + (size_t)cw * (TC_A_STAGE / 2)));
+            const uint64_t db = gmma_desc(slot + (uint32_t)w * TC_A_STAGE);
+#pragma unroll
+            for (int k = 0; k < TC_BK / 16; ++k)
+              wgmma_n128<F16, 0>(accA, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), ((kb + w) | k) != 0 ? 1u : 0u);
+          }
           wgmma_commit();
-          wgmma_wait<0>();
+          wgmma_wait<1>();                                         // the previous group (a W3 slot, or B(c-1)'s last k-block) has retired
           acc_fence<64>(accA);
-          if (signal) mbar_arrive(&empty[stage]);
+          if (prev >= 0) release(prev);
+          prev = stage;
+          if (xpend >= 0) { release_x(xpend); xpend = -1; }
           if (++stage == p.slots) { stage = 0; phase ^= 1; }
         }
+        wgmma_wait<0>();
+        acc_fence<64>(accA);
+        release(prev);
+        prev = -1;
         if (c == p.nch - 1 && signal) mbar_arrive(t2_empty);
         // ---- E(c): rows r, r + 8 of this thread, columns c*128 + 8j + 2 (lane % 4) + {0, 1} ----
+        mbar_wait(&x_full[xb], (uint32_t)((q >> 1) & 1));          // x_c has landed (and the buffer is free)
+        const uint32_t sXw = smem_u32(sX + (size_t)xb * BN_X_BYTES + (size_t)cw * (TC_A_STAGE / 2));   // this warpgroup's 64 rows
+        const float2* b3 = reinterpret_cast<const float2*>(p.b3 + c * 128) + (lane & 3);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int r = warp * 16 + (lane >> 2) + 8 * h;          // row in this warpgroup's 64-row slab
+        for (int j = 0; j < 16; ++j) {
+          const float2 b = __ldg(b3 + 4 * j);                      // columns c*128 + 8j + 2 (lane % 4) + {0, 1}: shared by both rows
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int col = c * 128 + 8 * j + 2 * (lane & 3);
-            uint32_t pk = 0u;
-            if (!zero[h]) {
-              const float2 b = __ldg(reinterpret_cast<const float2*>(p.b3 + col));
-              float v0 = b.x + accA[4 * j + 2 * h], v1 = b.y + accA[4 * j + 2 * h + 1];
-              if (p.has_res) {
-                const float2 rr = unpack2<F16>(__ldg(reinterpret_cast<const uint32_t*>((const uint16_t*)p.x + m[h] * p.Cexp + col)));
-                v0 += rr.x; v1 += rr.y;
-              }
-              pk = pack2<F16>(apply_act(v0, 1), apply_act(v1, 1));
-            }
-            if (valid[h]) *reinterpret_cast<uint32_t*>((uint16_t*)p.xo + m[h] * p.Cexp + col) = pk;
+          for (int h = 0; h < 2; ++h) {
+            const int r = warp * 16 + (lane >> 2) + 8 * h;        // row in this warpgroup's 64-row slab
             // A-operand layout: k-block j / 8, 16-byte chunk (j % 8) ^ (r % 8) of row r, element pair 2 (lane % 4)
-            *reinterpret_cast<uint32_t*>(sXw + (size_t)(j >> 3) * (TC_A_STAGE / 2) + r * 128 + ((((j & 7) ^ (r & 7))) << 4) + 4 * (lane & 3)) = pk;
+            const uint32_t a = sXw + (uint32_t)(j >> 3) * TC_A_STAGE + (uint32_t)r * 128u + ((uint32_t)((j & 7) ^ (r & 7)) << 4) + 4u * (lane & 3);
+            float v0 = b.x + accA[4 * j + 2 * h], v1 = b.y + accA[4 * j + 2 * h + 1];
+            if (p.has_res) {
+              const float2 rr = unpack2<F16>(lds32(a));
+              v0 += rr.x; v1 += rr.y;
+            }
+            const uint32_t pk = pack2<F16>(apply_act(v0, 1), apply_act(v1, 1));
+            sts32(a, zero[h] ? 0u : pk);                           // halo rows (and rows >= M) are zero
           }
         }
         fence_async_smem();
         named_barrier_sync(1 + cw, 128);                           // the whole x' chunk of this warpgroup is staged
+        if (t == 0) {
+          const int row = tile * TC_BM + cw * 64;
+#pragma unroll
+          for (int kb = 0; kb < 2; ++kb)
+            tma_store_2d(&tmXo, sX + (size_t)xb * BN_X_BYTES + (size_t)kb * TC_A_STAGE + (size_t)cw * (TC_A_STAGE / 2), c * 128 + kb * TC_BK, row);
+          bulk_commit();
+        }
         // ---- B(c) ----
         for (int kb = 0; kb < 2; ++kb) {
           mbar_wait(&full[stage], phase);
-          const uint64_t da = gmma_desc(smem_u32(sXw + (size_t)kb * (TC_A_STAGE / 2)));
+          const uint64_t da = gmma_desc(sXw + (uint32_t)kb * TC_A_STAGE);
           const uint64_t db = gmma_desc(smem_u32(sRing + (size_t)stage * p.slot_bytes));
           acc_fence<CMID / 2>(accB);
           wgmma_fence();
@@ -549,29 +607,36 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
           for (int k = 0; k < TC_BK / 16; ++k)
             wgmma_tile<CMID, F16, 0>(accB, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | kb | k) != 0 ? 1u : 0u);
           wgmma_commit();
-          wgmma_wait<0>();                                         // also: x' may be overwritten by the next chunk
+          wgmma_wait<1>();
           acc_fence<CMID / 2>(accB);
-          if (signal) mbar_arrive(&empty[stage]);
+          if (prev >= 0) release(prev);
+          prev = stage;
           if (++stage == p.slots) { stage = 0; phase ^= 1; }
         }
-        named_barrier_sync(1 + cw, 128);
+        xpend = xb;
       }
+      wgmma_wait<0>();
+      acc_fence<CMID / 2>(accB);
+      release(prev);
+      prev = -1;
+      release_x(xpend);
+      xpend = -1;
       // ---- t1 = relu(accB + b1), halo rows zero ----
+      const float2* b1 = reinterpret_cast<const float2*>(p.b1) + (lane & 3);
+      uint32_t* t1row[2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (!valid[h]) continue;
+      for (int h = 0; h < 2; ++h) t1row[h] = reinterpret_cast<uint32_t*>((uint16_t*)p.t1 + m[h] * CMID) + (lane & 3);
 #pragma unroll
-        for (int j = 0; j < CMID / 8; ++j) {
-          const int col = 8 * j + 2 * (lane & 3);
-          uint32_t pk = 0u;
-          if (!zero[h]) {
-            const float2 b = __ldg(reinterpret_cast<const float2*>(p.b1 + col));
-            pk = pack2<F16>(apply_act(b.x + accB[4 * j + 2 * h], 1), apply_act(b.y + accB[4 * j + 2 * h + 1], 1));
-          }
-          *reinterpret_cast<uint32_t*>((uint16_t*)p.t1 + m[h] * CMID + col) = pk;
+      for (int j = 0; j < CMID / 8; ++j) {
+        const float2 b = __ldg(b1 + 4 * j);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const uint32_t pk = pack2<F16>(apply_act(b.x + accB[4 * j + 2 * h], 1), apply_act(b.y + accB[4 * j + 2 * h + 1], 1));
+          if (valid[h]) t1row[h][4 * j] = zero[h] ? 0u : pk;
         }
       }
     }
+    if (t == 0) bulk_wait0();                                      // xo's stores are complete before the CTA exits
   }
 }
 
@@ -808,7 +873,7 @@ int launch_conv_tc(const TcPlan* pl, const ConvArgs& a, cudaStream_t s) {
 
 // ---- fused bottleneck tail (k_bneck_tc) ------------------------------------------------------------------------------
 struct BnPlan {
-  CUtensorMap tmT2, tmXd, tmW3, tmW1;
+  CUtensorMap tmT2, tmXd, tmW3, tmW1, tmX;                         // tmX: the residual, read by TMA in 128-row boxes
   int sms, Cmid, Cd, slots;
   uint32_t slot_bytes;
   size_t smem_bytes;
@@ -835,7 +900,7 @@ int bneck_plan_create(const BneckArgs& a, int max_batch, BnPlan** out) {
   pl->Cmid = a.Cmid; pl->Cd = a.Cd;
   const int kbA = (a.Cmid + a.Cd) / 64;
   pl->slot_bytes = (uint32_t)(a.Cmid * 128 > (int)TC_A_STAGE ? a.Cmid * 128 : (int)TC_A_STAGE);
-  const size_t fixed = 1024 /*align*/ + (2 * TC_MAX_STAGES + 2) * 8 /*barriers*/ + (size_t)kbA * TC_A_STAGE + 2 * TC_A_STAGE;
+  const size_t fixed = 1024 /*align*/ + (2 * TC_MAX_STAGES + 6) * 8 /*barriers*/ + (size_t)kbA * TC_A_STAGE + 2 * BN_X_BYTES;
   int slots = (int)((TC_SMEM_MAX - fixed) / pl->slot_bytes);
   pl->slots = slots > TC_MAX_STAGES ? TC_MAX_STAGES : slots;
   pl->smem_bytes = fixed + (size_t)pl->slots * pl->slot_bytes;
@@ -845,6 +910,8 @@ int bneck_plan_create(const BneckArgs& a, int max_batch, BnPlan** out) {
   if (s == YB_OK) s = make_map(&pl->tmT2, a.t2, (uint64_t)a.Cmid, rows, TC_BM, f16);
   pl->tmXd = pl->tmT2;                                             // placeholder without a folded branch
   if (s == YB_OK && a.Cd) s = make_map(&pl->tmXd, a.xd, (uint64_t)a.Cd, rows, TC_BM, f16);
+  pl->tmX = pl->tmT2;                                              // placeholder with a folded branch (no residual read)
+  if (s == YB_OK && !a.Cd) s = make_map(&pl->tmX, a.x, (uint64_t)a.Cexp, rows, TC_BM, f16);
   if (s == YB_OK) s = make_map(&pl->tmW3, a.w3, (uint64_t)(a.Cmid + a.Cd), (uint64_t)a.Cexp, 128, f16);
   if (s == YB_OK) s = make_map(&pl->tmW1, a.w1, (uint64_t)a.Cexp, (uint64_t)a.Cmid, (uint32_t)a.Cmid, f16);
   int dev = 0;
@@ -866,7 +933,10 @@ int launch_bneck_tc(const BnPlan* pl, const BneckArgs& a, cudaStream_t s) {
   p.m_tiles = (int)((p.M + TC_BM - 1) / TC_BM);
   p.Cexp = a.Cexp; p.nch = a.Cexp / 128; p.kbT = a.Cmid / 64; p.kbA = (a.Cmid + pl->Cd) / 64; p.has_res = pl->Cd ? 0 : 1;
   p.slots = pl->slots; p.slot_bytes = pl->slot_bytes;
-  p.g = a.g; p.b3 = a.b3; p.b1 = a.b1; p.x = a.x; p.xo = a.xo; p.t1 = a.t1;
+  p.g = a.g; p.b3 = a.b3; p.b1 = a.b1; p.t1 = a.t1;
+  // xo is written by TMA stores of [64 rows x 64 channels]; the map ends at this launch's last row, so rows >= M stay untouched
+  CUtensorMap tmXo;
+  YB_PROPAGATE(make_map(&tmXo, a.xo, (uint64_t)a.Cexp, (uint64_t)p.M, 64, a.act_dt == DT_F16));
   static const bool pdl = getenv("YOLACT_B200_NO_PDL") == nullptr;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)(p.m_tiles < pl->sms ? p.m_tiles : pl->sms)); cfg.blockDim = dim3(TC_THREADS);
@@ -875,7 +945,7 @@ int launch_bneck_tc(const BnPlan* pl, const BneckArgs& a, cudaStream_t s) {
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-  YB_CHECK_CUDA(with_bneck_kernel(a.act_dt == DT_F16, pl->Cmid, [&](auto k) { return cudaLaunchKernelEx(&cfg, k, pl->tmT2, pl->tmXd, pl->tmW3, pl->tmW1, p); }));
+  YB_CHECK_CUDA(with_bneck_kernel(a.act_dt == DT_F16, pl->Cmid, [&](auto k) { return cudaLaunchKernelEx(&cfg, k, pl->tmT2, pl->tmXd, pl->tmW3, pl->tmW1, pl->tmX, tmXo, p); }));
   YB_CHECK_LAUNCH();
   return YB_OK;
 }
