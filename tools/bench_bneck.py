@@ -76,7 +76,7 @@ def profile_rows(arch, size, batch, precision, forwards, fuse):
     os.environ.pop('YOLACT_B200_NO_FUSE', None)
     ops = {}
     for r in rows:
-        o = ops.setdefault(int(r['op']), {k: int(r[k]) for k in ('op', 'kind', 'tc', 'cin', 'cout', 'k', 'stride', 'h_out', 'batch')})
+        o = ops.setdefault(int(r['op']), dict({k: int(v) for k, v in r.items() if k not in ('forward', 'ms', 'gflop')}, gflop=float(r['gflop'])))
         o['ms'] = o.get('ms', 0.0) + float(r['ms']) / forwards
     del net, eng
     torch.cuda.empty_cache()

@@ -9,19 +9,31 @@
 //                 128B-swizzled, into a ring of shared-memory stages (mbarrier full / empty)
 //   warpgroups 1, 2  consumers: each owns 64 rows of the 128 x BN tile and issues wgmma.m64nBNk16 over the
 //                 staged operands, one k-block in flight while the previous one retires; then the epilogue
-//                 straight from the accumulator registers: + folded-BN bias, + residual, ReLU / GELU, clamp /
-//                 pack, halo zeroing (or dense fp32 rows)
+//                 (+ folded-BN bias, + residual, ReLU / GELU, clamp / pack, halo zeroing, or dense fp32 rows)
+//                 through shared memory, see "staged epilogue" below
 // Tiles are scheduled round-robin over the persistent grid, the N tiles of one M tile adjacent so the A tile
 // is shared through L2.  The tile width BN is a template parameter (wgmma encodes N in the instruction).
 // Launches use programmatic dependent launch: the prologue (barrier set-up, descriptor prefetch) overlaps the
 // previous kernel's tail; every role passes griddep_wait() before it touches activations.
 //
+// Staged epilogue (convolutions; the weight-gradient GEMM stores its fp32 fragments directly).  Each consumer warpgroup owns two
+// 8 KiB staging buffers and writes its 64 x BN result one column segment at a time, alternating between them:
+//   16-bit haloed output   segments of 64 columns (a 32- and a 16-column segment finish a width that is not a multiple of 64), in
+//                          the layout of a TMA box of [64 rows][w columns] with the swizzle of its 2w-byte rows (128, 64 or 32 B),
+//                          so the fragment's 4-byte stores are bank-conflict free; one thread then stores the box with
+//                          cp.async.bulk.tensor.  The map ends at the launch's last row: rows >= M are never written.  Halo rows
+//                          are staged as zero.  With a residual, the same box of the residual is loaded into the buffer by TMA one
+//                          segment ahead; the epilogue reads it and writes the result in place.
+//   dense fp32 output      segments of 32 columns ([64 rows][128 B], 16-byte chunks swizzled by row); after a warpgroup barrier the
+//                          128 threads copy the valid rows out with 16-byte stores, a 128-byte row segment per 8 threads.
+// A buffer is written again only after the store that read it has finished reading (cp.async.bulk.wait_group.read before the
+// warpgroup barrier that precedes the next segment's store), so the consumers go straight on to the next tile's MMAs.
+//
 // Launch forms, selected per plan (tc_plan_create):
 //   pair      cluster of two CTAs on adjacent 128-row tiles of one N tile; each CTA loads half of every weight tile and multicasts
 //             it to both shared memories (TMA .multicast::cluster), the stage is recycled once the consumers of BOTH CTAs release it
-//   res_kb    residual added by the tensor core: BN/64 extra k-blocks of the residual against a shared-memory identity tile
 //
-// Environment switches (tooling / A-B runs only): YOLACT_B200_PAIR=1, YOLACT_B200_RESMMA=1, YOLACT_B200_NO_PDL, YOLACT_B200_BN=<n>.
+// Environment switches (tooling / A-B runs only): YOLACT_B200_PAIR=1, YOLACT_B200_NO_PDL, YOLACT_B200_BN=<n>.
 #include "layers.cuh"
 #include "wgmma.cuh"
 
@@ -39,7 +51,8 @@ constexpr int TC_THREADS = 384;                    // producer warpgroup + 2 con
 constexpr uint32_t TC_A_STAGE = TC_BM * TC_BK * 2;   // 16 KiB
 constexpr int TC_MAX_STAGES = 8;
 constexpr size_t TC_SMEM_MAX = 227 * 1024;
-constexpr uint32_t TC_EYE_BYTES = 64 * 128;        // res_kb: the 64 x 64 identity operand
+constexpr uint32_t TC_STG_BYTES = 64 * 128;        // one staging buffer: 64 rows x 128 B
+constexpr uint32_t TC_STG_TOTAL = 4 * TC_STG_BYTES;  // two per consumer warpgroup
 
 struct TcParams {
   long long M;            // rows to produce (B * plane)
@@ -60,14 +73,20 @@ struct TcParams {
   int gemm_kb_split;      // scheduling unit each; the partial tiles are added to `out` with atomics (out is zeroed by the caller)
   Geom g;
   const float* bias;
-  const void* residual;
+  int residual;           // out_mode 0: + the residual, loaded into the staging buffers by TMA (TcMaps::res)
   void* out;
 };
 
+// the staged epilogue's TMA maps, one per segment width (index 0: 64, 1: 32, 2: 16 columns; unused widths hold a placeholder)
+struct TcMaps {
+  CUtensorMap res[3];      // the residual, boxes of [64 rows][w columns]
+  CUtensorMap out[3];      // the 16-bit output, the same boxes; the map ends at the launch's last row
+};
+
 struct TcPlan {
-  CUtensorMap tmA, tmB, tmRes;
+  CUtensorMap tmA, tmB;
+  CUtensorMap tmRes[3];    // TcMaps::res, encoded once for the max-batch rows
   int BN, stages, pair;
-  int res_kb;              // > 0: the residual is added by the tensor core in BN/64 identity k-blocks (k_conv_tc<..., RES = true>)
   int sms;                 // SM count of the device the plan was created on
   int gemm;                // plain-GEMM plan (tc_plan_create_gemm)
   size_t smem_bytes;
@@ -122,6 +141,22 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
   asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void named_barrier_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
+__device__ __forceinline__ uint32_t lds32(uint32_t a) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
+__device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+__device__ __forceinline__ void sts64(uint32_t a, float x, float y) { asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory"); }
+__device__ __forceinline__ float4 lds128(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 // programmatic dependent launch: let the next grid's CTAs start their prologue / block until the previous grid's
 // memory is complete and visible (both are no-ops for a launch without the programmatic-serialization attribute)
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -195,47 +230,41 @@ __device__ __forceinline__ void kb_range(const TcParams& p, int i, int& kb0, int
   kb1 = min(kb0 + p.gemm_kb_split, p.kb_per_tap);
 }
 
-// epilogue of one accumulator row segment: columns col, col+1 of row m (this thread's fragment pair)
-template <bool F16>
-__device__ __forceinline__ void store_pair(const TcParams& p, float a0, float a1, long long m, int col, bool halo, long long dense_row) {
-  if (p.out_mode == 2) {                                           // plain fp32 row-major [M][Cout_pad], no bias / activation
-    float2* o = reinterpret_cast<float2*>((float*)p.out + m * p.Cout_pad + col);
-    if (p.accumulate) atomicAdd(o, make_float2(a0, a1));
-    else *o = make_float2(a0, a1);
-    return;
-  }
-  if (p.out_mode == 0 && halo) {
-    *reinterpret_cast<uint32_t*>((uint16_t*)p.out + m * p.Cout + col) = 0u;
-    return;
-  }
-  if (halo) return;
-  const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
-  float v0 = b.x + a0, v1 = b.y + a1;
-  if (p.out_mode == 0) {
-    if (p.residual) {
-      const float2 r = unpack2<F16>(__ldg(reinterpret_cast<const uint32_t*>((const uint16_t*)p.residual + m * p.Cout + col)));
-      v0 += r.x; v1 += r.y;
-    }
-    v0 = apply_act(v0, p.relu); v1 = apply_act(v1, p.relu);
-    *reinterpret_cast<uint32_t*>((uint16_t*)p.out + m * p.Cout + col) = pack2<F16>(v0, v1);
-  } else {
-    v0 = apply_act(v0, p.relu); v1 = apply_act(v1, p.relu);
-    *reinterpret_cast<float2*>((float*)p.out + dense_row * p.Cout_pad + col) = make_float2(v0, v1);
-  }
-}
+// Column segments of a BN-wide tile in the staged epilogue.  16-bit output: 64 columns each, then at most one of 32 and one of 16
+// (176 = 64 + 64 + 32 + 16).  fp32 output: 32 columns each, the last one 16 when BN is an odd multiple of 16.
+template <int BN> struct Segs16 {
+  static constexpr int n64 = BN / 64, rem = BN % 64;
+  static constexpr int count = n64 + (rem >= 32 ? 1 : 0) + (rem % 32 != 0 ? 1 : 0);
+  static constexpr int width(int s) { return s < n64 ? 64 : (s == n64 && rem >= 32) ? 32 : 16; }
+  static constexpr int base(int s) { return s < n64 ? 64 * s : 64 * n64 + (s == n64 || rem < 32 ? 0 : 32); }
+  static constexpr int of(int col) { return col < 64 * n64 ? col / 64 : (rem >= 32 && col < 64 * n64 + 32) ? n64 : count - 1; }
+};
+// TcMaps index of a segment width
+__host__ __device__ constexpr int seg_map(int w) { return w == 64 ? 0 : w == 32 ? 1 : 2; }
 
-template <bool F16, bool MNB, int BN, bool RES>
+// Byte offset of 16-bit element cc of row r in a TMA box of [64 rows][w columns] with the swizzle of its 2w-byte rows: the 16-byte
+// chunk index is XORed with address bits 7.. (SWIZZLE_128B / 64B / 32B).  A warp's fragment stores of one column pair cover eight
+// rows; the XOR puts them in distinct banks.
+__device__ __forceinline__ uint32_t stg_off16(int r, int cc, int w) {
+  const int rb = r * 2 * w;
+  return (uint32_t)(rb + ((((cc >> 3) ^ (rb >> 7)) & (w / 8 - 1)) << 4) + (cc & 7) * 2);
+}
+// fp32 staging: row r at r * 128 B, 16-byte chunk (cc / 4) ^ (r % 8)
+__device__ __forceinline__ uint32_t stg_off32(int r, int cc) { return (uint32_t)(r * 128 + ((((cc >> 2) ^ r) & 7) << 4) + (cc & 3) * 4); }
+
+template <bool F16, bool MNB, int BN>
 __global__ void __launch_bounds__(TC_THREADS, 1)
-k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmRes,
+k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ TcMaps maps,
           const TcParams p) {
   constexpr uint32_t B_STAGE = (uint32_t)BN * TC_BK * 2;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);     // SWIZZLE_128B needs 1024B alignment
   uint8_t* sA = smem;                                                               // [stages][128 rows x 128 B]
   uint8_t* sB = smem + (size_t)p.stages * TC_A_STAGE;                               // [stages][BN rows x 128 B] (MN-major: BN/64 boxes)
-  uint8_t* sEye = sB + (size_t)p.stages * B_STAGE;                                  // res_kb: [64 rows x 128 B] identity operand
-  uint64_t* full = reinterpret_cast<uint64_t*>(sEye + (RES ? TC_EYE_BYTES : 0u));
+  uint8_t* sStg = sB + (size_t)p.stages * B_STAGE;                                  // convolutions: [2 warpgroups][2 buffers][8 KiB]
+  uint64_t* full = reinterpret_cast<uint64_t*>(sStg + (MNB ? 0u : TC_STG_TOTAL));
   uint64_t* empty = full + TC_MAX_STAGES;
+  uint64_t* res_full = empty + TC_MAX_STAGES;                                       // [2 warpgroups][2 buffers]: the residual box landed
 
   const int wg = threadIdx.x >> 7;
   const uint32_t rank = p.pair ? cluster_ctarank() : 0u;
@@ -244,30 +273,16 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     // empty: one arrive per consumer warp -- of both CTAs in the pair form, whose weight half lands in both shared memories
     for (int i = 0; i < TC_MAX_STAGES; ++i) { mbar_init(&full[i], 1); mbar_init(&empty[i], p.pair ? 16 : 8); }
+    for (int i = 0; i < 4; ++i) mbar_init(&res_full[i], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (RES && wg > 0) {
-    // identity operand (K-major, 128B-swizzled): row n holds 1.0 at element n, which lives in 16-byte chunk (n / 8) ^ (n & 7)
-    const int t = (int)threadIdx.x - 128, n = t >> 2;              // 256 threads: four per row, two chunks each
-    const uint32_t one = F16 ? 0x3C00u : 0x3F80u;
-#pragma unroll
-    for (int q = 0; q < 2; ++q) {
-      const int ch = (t & 3) * 2 + q;
-      uint4 v = make_uint4(0u, 0u, 0u, 0u);
-      if (ch == (n >> 3)) {
-        const int e = n & 7;
-        const uint32_t w = (e & 1) ? (one << 16) : one;
-        if ((e >> 1) == 0) v.x = w; else if ((e >> 1) == 1) v.y = w; else if ((e >> 1) == 2) v.z = w; else v.w = w;
-      }
-      *reinterpret_cast<uint4*>(sEye + n * 128 + ((ch ^ (n & 7)) << 4)) = v;
-    }
-    fence_async_smem();
   }
   if (p.pair) cluster_sync_all(); else __syncthreads();            // pair: the peer's barriers are initialised too
   griddep_launch_dependents();
 
+  // the producer warpgroup needs few registers: the consumers take them (BN = 256: 128 accumulators and the staged epilogue)
   if (wg == 0) {
     // ================= TMA producer =================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
     if (threadIdx.x == 0) {
       griddep_wait();
       int stage = 0; uint32_t phase = 0;
@@ -299,16 +314,11 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           }
           if (++stage == p.stages) { stage = 0; phase ^= 1; }
         }
-        for (int j = 0; j < (RES ? BN / 64 : 0); ++j) {             // residual k-blocks: [128 rows x 64 channels] of the residual (A slot only)
-          mbar_wait(&empty[stage], phase ^ 1);
-          mbar_expect_tx(&full[stage], TC_A_STAGE);
-          tma_load_2d(sA + (size_t)stage * TC_A_STAGE, &tmRes, n0 + j * TC_BK, m0, &full[stage]);
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
       }
     }
   } else {
     // ================= consumers: warpgroup c owns rows 64c .. 64c+63 of every tile =================
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
     const int c = wg - 1;
     const int t = threadIdx.x & 127, warp = t >> 5, lane = t & 31;
     const bool signal = lane == 0;
@@ -323,6 +333,16 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
     float acc[BN / 2];
     int stage = 0; uint32_t phase = 0;
     int m_tile, n_tile;
+    uint8_t* stg = sStg + (size_t)c * 2 * TC_STG_BYTES;             // this warpgroup's two staging buffers
+    uint32_t q = 0;                                                 // segments staged so far: buffer q & 1
+    // the residual box of 16-bit segment s of tile (mt, nt) into the buffer of segment qq (thread 0 of the warpgroup)
+    auto load_res = [&](uint32_t qq, int mt, int nt, int s) {
+      const int w = Segs16<BN>::width(s);
+      uint64_t* bar = &res_full[2 * c + (qq & 1)];
+      mbar_expect_tx(bar, 64u * 2u * (uint32_t)w);
+      tma_load_2d(stg + (qq & 1) * TC_STG_BYTES, &maps.res[seg_map(w)], nt * BN + Segs16<BN>::base(s), mt * TC_BM + c * 64, bar);
+    };
+    if (!MNB && p.residual && t == 0 && tile_at(p, 0, m_tile, n_tile)) load_res(0, m_tile, n_tile, 0);
     for (int i = 0; tile_at(p, i, m_tile, n_tile); ++i) {
       int kb0, kb1;
       kb_range(p, i, kb0, kb1);
@@ -346,49 +366,116 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
         prev = stage;
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
-      if constexpr (RES) {
-        // D[:, 64j .. 64j+63] += R_j * I: columns 64j .. 64j+63 are the fragment registers acc[32j .. 32j+31] (j a compile-time index)
-        const uint64_t de = gmma_desc(smem_u32(sEye));
-#pragma unroll
-        for (int j = 0; j < BN / 64; ++j) {
-          mbar_wait(&full[stage], phase);
-          const uint64_t da = gmma_desc(smem_u32(sA + (size_t)stage * TC_A_STAGE + (size_t)c * (TC_A_STAGE / 2)));
-          acc_fence<BN / 2>(acc);
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < TC_BK / 16; ++k) wgmma_n64<F16, 0>(acc + 32 * j, da + (uint64_t)(k * 2), de + (uint64_t)(k * 2), 1u);
-          wgmma_commit();
-          wgmma_wait<1>();
-          acc_fence<BN / 2>(acc);
-          release(prev);
-          prev = stage;
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
-      }
       wgmma_wait<0>();
       acc_fence<BN / 2>(acc);
       if (prev >= 0) release(prev);
 
-      // ---- epilogue straight from the fragment: rows r and r + 8, columns 8j + 2 (lane % 4) + {0, 1} ----
-      const int col0 = n_tile * BN + 2 * (lane & 3);               // gemm: N tile n of tap t is column t * Nper + (n % gemm_ntile_tap) * BN
+      // ---- epilogue: this thread's fragment holds rows r and r + 8 of the warpgroup's 64, columns 8j + 2 (lane % 4) + {0, 1} ----
+      const int n0 = n_tile * BN;                                  // gemm: N tile n of tap t is column t * Nper + (n % gemm_ntile_tap) * BN
+      const int row0 = m_tile * TC_BM + c * 64;
+      const int r0 = warp * 16 + (lane >> 2);
+      if constexpr (MNB) {                                         // weight-gradient GEMM: plain fp32 [M][Cout_pad], stored or added
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const long long m = (long long)m_tile * TC_BM + c * 64 + warp * 16 + (lane >> 2) + 8 * h;
-        if (m >= p.M) continue;
-        bool halo = false;
-        long long dense_row = 0;
-        if (p.out_mode != 2) {
-          const int plane = p.g.plane();
-          const int img = (int)(m / plane);
-          const int pos = (int)(m - (long long)img * plane);
-          const int y = pos / p.g.Wp(), x = pos - y * p.g.Wp();
-          halo = y == 0 || y == p.g.H + 1 || x == 0 || x == p.g.W + 1;
-          dense_row = ((long long)img * p.g.H + (y - 1)) * p.g.W + (x - 1);
+        for (int h = 0; h < 2; ++h) {
+          const long long m = (long long)row0 + r0 + 8 * h;
+          if (m >= p.M) continue;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            float2* o = reinterpret_cast<float2*>((float*)p.out + m * p.Cout_pad + n0 + 8 * j + 2 * (lane & 3));
+            const float2 v = make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            if (p.accumulate) atomicAdd(o, v);
+            else *o = v;
+          }
         }
+      } else if (p.out_mode == 0) {
+        // ---- 16-bit haloed rows: staged per segment, stored by TMA ----
+        bool zero[2];                                              // halo rows are zero (rows >= M too; the store clips them)
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) store_pair<F16>(p, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], m, col0 + 8 * j, halo, dense_row);
+        for (int h = 0; h < 2; ++h) {
+          const long long m = (long long)row0 + r0 + 8 * h;
+          zero[h] = true;
+          if (m < p.M) {
+            const int pos = (int)(m % p.g.plane());
+            const int y = pos / p.g.Wp(), x = pos - y * p.g.Wp();
+            zero[h] = y == 0 || y == p.g.H + 1 || x == 0 || x == p.g.W + 1;
+          }
+        }
+        const float2* bias = reinterpret_cast<const float2*>(p.bias + n0) + (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {                         // j is a compile-time index: the segment arithmetic folds away
+          const int s = Segs16<BN>::of(8 * j), w = Segs16<BN>::width(s), sb = Segs16<BN>::base(s);
+          uint8_t* buf = stg + (q & 1) * TC_STG_BYTES;
+          if (p.residual && 8 * j == sb) mbar_wait(&res_full[2 * c + (q & 1)], (q >> 1) & 1);
+          const float2 b = __ldg(bias + 4 * j);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const uint32_t a = smem_u32(buf) + stg_off16(r0 + 8 * h, 8 * j - sb + 2 * (lane & 3), w);
+            float v0 = b.x + acc[4 * j + 2 * h], v1 = b.y + acc[4 * j + 2 * h + 1];
+            if (p.residual) {
+              const float2 rr = unpack2<F16>(lds32(a));
+              v0 += rr.x; v1 += rr.y;
+            }
+            const uint32_t pk = pack2<F16>(apply_act(v0, p.relu), apply_act(v1, p.relu));
+            sts32(a, zero[h] ? 0u : pk);
+          }
+          if (8 * j + 8 == sb + w) {                               // the segment is complete
+            fence_async_smem();
+            if (t == 0) bulk_wait_read0();                         // the previous segment's store has read the other buffer
+            named_barrier_sync(1 + c, 128);
+            if (t == 0) {
+              tma_store_2d(&maps.out[seg_map(w)], buf, n0 + sb, row0);
+              bulk_commit();
+              if (p.residual) {                                    // the next segment's residual box, into the other buffer
+                int mt, nt;
+                if (s + 1 < Segs16<BN>::count) load_res(q + 1, m_tile, n_tile, s + 1);
+                else if (tile_at(p, i + 1, mt, nt)) load_res(q + 1, mt, nt, 0);
+              }
+            }
+            ++q;
+          }
+        }
+      } else {
+        // ---- dense fp32 rows (halo rows skipped): staged per segment, copied out with 16-byte stores ----
+        // thread t copies 16-byte chunk t % 8 of rows t / 8 + 16k; drow: their dense rows, -1 for halo rows and rows >= M
+        long long drow[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const long long m = (long long)row0 + (t >> 3) + 16 * k;
+          drow[k] = -1;
+          if (m < p.M) {
+            const int plane = p.g.plane();
+            const int img = (int)(m / plane);
+            const int pos = (int)(m - (long long)img * plane);
+            const int y = pos / p.g.Wp(), x = pos - y * p.g.Wp();
+            if (!(y == 0 || y == p.g.H + 1 || x == 0 || x == p.g.W + 1)) drow[k] = ((long long)img * p.g.H + (y - 1)) * p.g.W + (x - 1);
+          }
+        }
+        const float2* bias = reinterpret_cast<const float2*>(p.bias + n0) + (lane & 3);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const int sb = (8 * j) / 32 * 32, w = BN - sb < 32 ? BN - sb : 32;
+          const uint32_t buf = smem_u32(stg + (q & 1) * TC_STG_BYTES);
+          const float2 b = __ldg(bias + 4 * j);
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            sts64(buf + stg_off32(r0 + 8 * h, 8 * j - sb + 2 * (lane & 3)), apply_act(b.x + acc[4 * j + 2 * h], p.relu),
+                  apply_act(b.y + acc[4 * j + 2 * h + 1], p.relu));
+          if (8 * j + 8 == sb + w) {
+            // every thread has staged this segment and finished copying out the previous one from the other buffer
+            named_barrier_sync(1 + c, 128);
+            const int ch = t & 7;
+            if (ch < w / 4) {
+#pragma unroll
+              for (int k = 0; k < 4; ++k)
+                if (drow[k] >= 0)
+                  *reinterpret_cast<float4*>((float*)p.out + drow[k] * p.Cout_pad + n0 + sb + 4 * ch) = lds128(buf + stg_off32((t >> 3) + 16 * k, 4 * ch));
+            }
+            ++q;
+          }
+        }
       }
     }
+    if (!MNB && t == 0) bulk_wait0();                              // the TMA stores are complete before the CTA exits
   }
   if (p.pair) cluster_sync_all();                                  // neither CTA leaves while the peer may still signal its barriers
 }
@@ -422,17 +509,6 @@ struct BnParams {
   const float* b1;
   void* t1;
 };
-
-__device__ __forceinline__ void named_barrier_sync(int id, int threads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory"); }
-__device__ __forceinline__ uint32_t lds32(uint32_t a) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
-__device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 constexpr uint32_t BN_X_BYTES = 2 * TC_A_STAGE;                  // one x buffer: 128 rows x 128 channels
 
@@ -657,6 +733,7 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
+// 2D map over a 16-bit [rows][inner] matrix; the swizzle spans a box row: 128 B for 64 elements, 64 B for 32, 32 B for 16
 static int make_map(CUtensorMap* map, const void* base, uint64_t inner, uint64_t rows, uint32_t box_rows, bool f16,
                     uint32_t box_inner = TC_BK, uint64_t row_stride = 0) {
   EncodeTiledFn enc = get_encode();
@@ -665,9 +742,9 @@ static int make_map(CUtensorMap* map, const void* base, uint64_t inner, uint64_t
   const cuuint64_t strides[1] = {(row_stride ? row_stride : inner) * 2};
   const cuuint32_t box[2] = {box_inner, box_rows};
   const cuuint32_t estr[2] = {1, 1};
+  const CUtensorMapSwizzle swz = box_inner == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : box_inner == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
   CUresult r = enc(map, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                   CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   YB_REQUIRE(r == CUDA_SUCCESS, YB_ERR_CUDA, "cuTensorMapEncodeTiled failed (%d) inner=%llu rows=%llu box_rows=%u", (int)r,
              (unsigned long long)inner, (unsigned long long)rows, box_rows);
   return YB_OK;
@@ -690,29 +767,25 @@ bool tc_overlapping_rows_ok() {
 }
 
 // call f(kernel) with the instantiation for (f16, MN-major B, BN)
-// call f(kernel) with the instantiation for (f16, MN-major B, BN, residual through the tensor core)
-template <class F> static cudaError_t with_kernel(bool f16, bool mnb, int bn, bool res, F&& f) {
+template <class F> static cudaError_t with_kernel(bool f16, bool mnb, int bn, F&& f) {
 #define YB_TC_CASE(N)                                                              \
   case N:                                                                          \
-    return f16 ? f(k_conv_tc<true, false, N, false>) : f(k_conv_tc<false, false, N, false>);
-#define YB_TC_CASE_RES(N)                                                          \
-  case N:                                                                          \
-    return f16 ? f(k_conv_tc<true, false, N, true>) : f(k_conv_tc<false, false, N, true>);
+    return f16 ? f(k_conv_tc<true, false, N>) : f(k_conv_tc<false, false, N>);
 #define YB_TC_CASE_MN(N)                                                           \
   case N:                                                                          \
-    return f16 ? f(k_conv_tc<true, true, N, false>) : f(k_conv_tc<false, true, N, false>);
+    return f16 ? f(k_conv_tc<true, true, N>) : f(k_conv_tc<false, true, N>);
   if (mnb) {
     switch (bn) { YB_TC_CASE_MN(64) YB_TC_CASE_MN(128) YB_TC_CASE_MN(256) }
-  } else if (res) {
-    switch (bn) { YB_TC_CASE_RES(64) YB_TC_CASE_RES(128) YB_TC_CASE_RES(192) YB_TC_CASE_RES(256) }
   } else {
     switch (bn) { YB_TC_CASE(16) YB_TC_CASE(32) YB_TC_CASE(64) YB_TC_CASE(96) YB_TC_CASE(128) YB_TC_CASE(176) YB_TC_CASE(192) YB_TC_CASE(256) }
   }
 #undef YB_TC_CASE
-#undef YB_TC_CASE_RES
 #undef YB_TC_CASE_MN
   return cudaErrorInvalidValue;
 }
+
+// does the 16-bit staged epilogue of a BN-wide tile have a segment of width w (Segs16)?
+static bool seg_width_used(int bn, int w) { return w == 64 ? bn >= 64 : w == 32 ? bn % 64 >= 32 : bn % 32 != 0; }
 
 // the tile widths with a kernel instantiation (wgmma.cuh), widest first
 static const int kTileWidths[] = {256, 192, 176, 128, 96, 64, 32, 16};
@@ -734,11 +807,11 @@ bool tc_supported(const ConvArgs& a) {
 }
 
 // per-device set-up and SM count; the kernel's dynamic shared-memory limit is raised for the plan's instantiation
-static int tc_device_setup(bool f16, bool mnb, int bn, bool res, int* sms) {
+static int tc_device_setup(bool f16, bool mnb, int bn, int* sms) {
   int dev = 0;
   YB_CHECK_CUDA(cudaGetDevice(&dev));
   // the instantiation's limit is the whole 227 KB: plans of different sizes share one instantiation
-  YB_CHECK_CUDA(with_kernel(f16, mnb, bn, res, [&](auto k) { return cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_MAX); }));
+  YB_CHECK_CUDA(with_kernel(f16, mnb, bn, [&](auto k) { return cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_MAX); }));
   YB_CHECK_CUDA(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
   YB_REQUIRE(*sms > 0, YB_ERR_CUDA, "cannot read the SM count");
   return YB_OK;
@@ -746,7 +819,7 @@ static int tc_device_setup(bool f16, bool mnb, int bn, bool res, int* sms) {
 
 static void plan_stages(TcPlan* pl) {
   const size_t per_stage = TC_A_STAGE + (size_t)pl->BN * TC_BK * 2;
-  const size_t fixed = 1024 /*align*/ + 2 * TC_MAX_STAGES * 8 /*barriers*/ + (pl->res_kb ? TC_EYE_BYTES : 0);
+  const size_t fixed = 1024 /*align*/ + (2 * TC_MAX_STAGES + 4) * 8 /*barriers*/ + (pl->gemm ? 0 : TC_STG_TOTAL);
   int stages = (int)((TC_SMEM_MAX - fixed) / per_stage);
   pl->stages = stages > TC_MAX_STAGES ? TC_MAX_STAGES : stages;
   pl->smem_bytes = (size_t)pl->stages * per_stage + fixed;
@@ -754,15 +827,13 @@ static void plan_stages(TcPlan* pl) {
 
 int tc_plan_create(const ConvArgs& a, int max_batch, TcPlan** out) {
   YB_REQUIRE(tc_supported(a), YB_ERR_UNSUPPORTED, "tc_plan_create: unsupported conv Cin=%d Cout_pad=%d", a.Cin, a.Cout_pad);
+  YB_REQUIRE(!a.residual || a.out_mode == 0, YB_ERR_UNSUPPORTED, "tc_plan_create: a residual needs the 16-bit haloed output");
   TcPlan* pl = new TcPlan();
   pl->gemm = 0;
   pl->BN = pick_bn(a.Cout_pad);
-  // The pair and residual-MMA forms are selected with YOLACT_B200_PAIR=1 / YOLACT_B200_RESMMA=1 (A-B runs; both are checked
-  // at every test shape); the default is one CTA per tile with the residual read in the epilogue.
+  // The pair form is selected with YOLACT_B200_PAIR=1 (A-B runs; it is checked at every test shape); the default is one CTA per tile.
   const char* e_pair = getenv("YOLACT_B200_PAIR");
-  const char* e_res = getenv("YOLACT_B200_RESMMA");
   pl->pair = (e_pair && atoi(e_pair) != 0) ? 1 : 0;
-  pl->res_kb = (e_res && atoi(e_res) != 0 && a.residual && a.out_mode == 0 && pl->BN % 64 == 0) ? pl->BN / 64 : 0;
   plan_stages(pl);
   const int Ktot = a.ntaps * a.Cin_pad;
   const int cout_alloc = (a.Cout_pad + 63) / 64 * 64;
@@ -770,9 +841,13 @@ int tc_plan_create(const ConvArgs& a, int max_batch, TcPlan** out) {
   int s = make_map(&pl->tmA, a.in, (uint64_t)a.Cin, (uint64_t)a.in_rows, TC_BM, f16, TC_BK, (uint64_t)a.in_row_stride);
   if (s == YB_OK) s = make_map(&pl->tmB, a.weight, (uint64_t)Ktot, (uint64_t)cout_alloc, (uint32_t)(pl->pair ? pl->BN / 2 : pl->BN), f16, TC_BK,
                                (uint64_t)a.w_ld);
-  pl->tmRes = pl->tmA;                                             // placeholder when the residual is not read by TMA
-  if (s == YB_OK && pl->res_kb) s = make_map(&pl->tmRes, a.residual, (uint64_t)a.Cout, (uint64_t)max_batch * a.g.plane(), TC_BM, f16);
-  if (s == YB_OK) s = tc_device_setup(f16, false, pl->BN, pl->res_kb != 0, &pl->sms);
+  for (int w : {64, 32, 16}) {                                     // the residual boxes of the tile's segment widths (placeholders otherwise)
+    CUtensorMap* m = &pl->tmRes[seg_map(w)];
+    *m = pl->tmA;
+    if (s == YB_OK && a.residual && seg_width_used(pl->BN, w))
+      s = make_map(m, a.residual, (uint64_t)a.Cout, (uint64_t)max_batch * a.g.plane(), 64, f16, (uint32_t)w);
+  }
+  if (s == YB_OK) s = tc_device_setup(f16, false, pl->BN, &pl->sms);
   if (s != YB_OK) { delete pl; return s; }
   *out = pl;
   return YB_OK;
@@ -780,7 +855,7 @@ int tc_plan_create(const ConvArgs& a, int max_batch, TcPlan** out) {
 
 void tc_plan_destroy(TcPlan* p) { delete p; }
 
-static int launch(const TcPlan* pl, const TcParams& p, bool f16, int grid, cudaStream_t s) {
+static int launch(const TcPlan* pl, const TcParams& p, const TcMaps& maps, bool f16, int grid, cudaStream_t s) {
   static const bool pdl = getenv("YOLACT_B200_NO_PDL") == nullptr;
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3((unsigned)grid); cfg.blockDim = dim3(TC_THREADS); cfg.dynamicSmemBytes = pl->smem_bytes; cfg.stream = s;
@@ -797,7 +872,7 @@ static int launch(const TcPlan* pl, const TcParams& p, bool f16, int grid, cudaS
     ++na;
   }
   cfg.attrs = attr; cfg.numAttrs = na;
-  YB_CHECK_CUDA(with_kernel(f16, pl->gemm != 0, pl->BN, pl->res_kb != 0, [&](auto k) { return cudaLaunchKernelEx(&cfg, k, pl->tmA, pl->tmB, pl->tmRes, p); }));
+  YB_CHECK_CUDA(with_kernel(f16, pl->gemm != 0, pl->BN, [&](auto k) { return cudaLaunchKernelEx(&cfg, k, pl->tmA, pl->tmB, maps, p); }));
   YB_CHECK_LAUNCH();
   return YB_OK;
 }
@@ -819,8 +894,7 @@ int tc_plan_create_gemm(const GemmArgs& g, TcPlan** out) {
   int s = make_map(&pl->tmA, g.a, (uint64_t)g.K, (uint64_t)g.M, TC_BM, f16, TC_BK, (uint64_t)g.lda);
   // B is read MN-major straight from the [Kb pixels][ldb channels] activations: boxes of [64 k-rows][64 channels]
   if (s == YB_OK) s = make_map(&pl->tmB, g.b, (uint64_t)g.Nper, (uint64_t)g.Kb, 64, f16, TC_BK, (uint64_t)g.ldb);
-  pl->tmRes = pl->tmA;
-  if (s == YB_OK) s = tc_device_setup(f16, true, bn, false, &pl->sms);
+  if (s == YB_OK) s = tc_device_setup(f16, true, bn, &pl->sms);
   if (s != YB_OK) { delete pl; return s; }
   *out = pl;
   return YB_OK;
@@ -844,9 +918,11 @@ int launch_gemm_tc(const TcPlan* pl, const GemmArgs& g, cudaStream_t s) {
   p.stages = pl->stages;
   p.Cout = p.Cout_pad = g.ntaps * g.Nper; p.relu = 0; p.out_mode = 2; p.accumulate = g.accumulate;
   p.g.H = 1 << 20; p.g.W = 1 << 20;
-  p.bias = nullptr; p.residual = nullptr; p.out = g.out;
+  p.bias = nullptr; p.residual = 0; p.out = g.out;
   const int total = p.m_tiles * p.n_tiles * p.gemm_splits;
-  return launch(pl, p, g.act_dt == DT_F16, total < pl->sms ? total : pl->sms, s);
+  TcMaps maps;                                                     // no staged epilogue: placeholders
+  for (int k = 0; k < 3; ++k) maps.res[k] = maps.out[k] = pl->tmA;
+  return launch(pl, p, maps, g.act_dt == DT_F16, total < pl->sms ? total : pl->sms, s);
 }
 
 int launch_conv_tc(const TcPlan* pl, const ConvArgs& a, cudaStream_t s) {
@@ -863,12 +939,21 @@ int launch_conv_tc(const TcPlan* pl, const ConvArgs& a, cudaStream_t s) {
   p.stages = pl->stages;
   p.Cout = a.Cout; p.Cout_pad = a.Cout_pad; p.relu = a.relu; p.out_mode = a.out_mode;
   p.g = a.g; p.bias = a.bias; p.out = a.out;
-  p.residual = pl->res_kb ? nullptr : a.residual;                 // res_kb: added by the tensor core, not in the epilogue
+  p.residual = a.residual != nullptr;
   p.gemm = 0; p.gemm_ntile_tap = 1; p.gemm_splits = 1;
   const int total = p.m_tiles * p.n_tiles;
   const int max_units = pl->pair ? pl->sms / 2 : pl->sms;
   const int units = total < max_units ? total : max_units;
-  return launch(pl, p, a.act_dt == DT_F16, pl->pair ? 2 * units : units, s);
+  // 16-bit output: TMA store boxes of the tile's segment widths; the maps end at this launch's last row, so rows >= M stay untouched
+  TcMaps maps;
+  for (int w : {64, 32, 16}) {
+    const int k = seg_map(w);
+    maps.res[k] = pl->tmRes[k];
+    maps.out[k] = pl->tmA;
+    if (a.out_mode == 0 && seg_width_used(pl->BN, w))
+      YB_PROPAGATE(make_map(&maps.out[k], a.out, (uint64_t)a.Cout, (uint64_t)p.M, 64, a.act_dt == DT_F16, (uint32_t)w));
+  }
+  return launch(pl, p, maps, a.act_dt == DT_F16, pl->pair ? 2 * units : units, s);
 }
 
 // ---- fused bottleneck tail (k_bneck_tc) ------------------------------------------------------------------------------

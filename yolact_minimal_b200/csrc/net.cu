@@ -846,7 +846,7 @@ extern "C" int yb_net_profile(yb_net* net, yb_prof_entry* out, int max_entries, 
   const size_t esz = dtype_size(net->act_dt);
   FILE* dump = nullptr;
   if (const char* path = getenv("YOLACT_B200_PROFILE_DUMP")) dump = fopen(path, "w");
-  if (dump) fprintf(dump, "forward,op,kind,tc,cin,cout,k,stride,h_out,batch,ms,gflop\n");
+  if (dump) fprintf(dump, "forward,op,kind,tc,cin,cout,k,stride,h_out,batch,ms,gflop,res,out_mode\n");
   for (size_t f = 0; f < net->prof_sets.size(); ++f) {
     auto& evs = net->prof_sets[f];
     const double B = net->prof_batch[f];
@@ -893,8 +893,8 @@ extern "C" int yb_net_profile(yb_net* net, yb_prof_entry* out, int max_entries, 
       }
       if (dump) {
         const ConvW* c = (o.kind == OP_CONV || o.kind == OP_BNECK) ? &net->convs[o.conv] : nullptr;
-        fprintf(dump, "%zu,%zu,%d,%d,%d,%d,%d,%d,%d,%d,%.5f,%.4f\n", f, i, (int)o.kind, o.tc ? 1 : 0, c ? c->Cin : 0, c ? c->Cout_pad : 0,
-                c ? c->k : 0, o.stride, c ? net->acts[o.in].H : 0, (int)B, ms, flops * 1e-9);
+        fprintf(dump, "%zu,%zu,%d,%d,%d,%d,%d,%d,%d,%d,%.5f,%.4f,%d,%d\n", f, i, (int)o.kind, o.tc ? 1 : 0, c ? c->Cin : 0, c ? c->Cout_pad : 0,
+                c ? c->k : 0, o.stride, c ? net->acts[o.in].H : 0, (int)B, ms, flops * 1e-9, o.res >= 0 ? 1 : 0, o.out_mode);
       }
       out[k].launches += (o.kind == OP_STEM ? 2 : 1);
       out[k].ms += ms; out[k].flops += flops; out[k].bytes += bytes;
