@@ -182,6 +182,26 @@ YB_API int yb_eval_ap(const yb_eval_params* p, const float* rec_score, const int
 YB_API int yb_val_aug(const uint8_t* img_bgr, int h, int w, int img_size, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Drawing -- the pixel work of utils/output_utils.py:308-369 (draw_img); the box, label and fps drawing stays on the host.
+ *   semantic = (sum_i m_i * (ids_i + 1)) mod num_colors     floor modulo (numpy %); num_colors = cfg.num_classes - 1
+ *   yb_draw_masks   out = rint(0.4f * palette[semantic] + 0.6f * img) per channel -- cv2.addWeighted(COLORS[semantic], 0.4,
+ *                   img, 0.6, 0) on uint8, every pixel (the background blends with palette[0]); one launch
+ *   yb_draw_cutout  cfg.cutout: out_total = semantic != 0 ? img : 255 ([h,w,3]); crop i = (m_i != 0 ? img : 255) over rows
+ *                   crop_yyxx[i] = (y1, y2, x1, x2) -> cols [x1, x2), written [y2-y1, x2-x1, 3] at out_crops + crop_off[i]
+ *                   (int64 byte offsets [n+1]).  A crop outside the image, or whose range crop_off[i] .. crop_off[i+1] does not
+ *                   hold exactly its 3 * area bytes, is skipped (nothing is written for it).
+ * img_bgr / out_* uint8 [h,w,3] (HWC, any channel order: channel c of the palette applies to channel c of the image);
+ * masks [n,h,w] with values {0,1} in the layouts of yb_mask_assemble (mask_fmt 0 uint8, 1 float32 -- 16-byte aligned, 2
+ * bit-packed words [n,h,ceil(w/32)]); ids int32 [n]; palette uint8 [num_colors,3].  n <= 4096, 1 <= num_colors <= 1024.
+ * All pointers are DEVICE pointers; asynchronous on stream.  out_bgr may alias img_bgr.
+ * ---------------------------------------------------------------------------------------- */
+YB_API int yb_draw_masks(const uint8_t* img_bgr, int h, int w, const void* masks, int mask_fmt, int n, const int32_t* ids,
+                         const uint8_t* palette, int num_colors, uint8_t* out_bgr, void* stream);
+YB_API int yb_draw_cutout(const uint8_t* img_bgr, int h, int w, const void* masks, int mask_fmt, int n, const int32_t* ids,
+                          int num_colors, const int32_t* crop_yyxx, const int64_t* crop_off, uint8_t* out_total,
+                          uint8_t* out_crops, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Network: ResNet-50/101 + FPN + ProtoNet + prediction heads (modules/resnet.py,
  * modules/yolact.py:12-164), eval forward.  Weights are handed over by their reference
  * state-dict names (SURVEY.md App. C); BatchNorm is folded at finalize time.

@@ -71,6 +71,8 @@ PROTOTYPES = {
     'yb_mask_iou_bits': (C.c_int, [vp, C.c_int, vp, C.c_int, C.c_int64, vp, vp]),
     'yb_box_iou': (C.c_int, [vp, C.c_int, vp, C.c_int, vp, vp]),
     'yb_mask_rle': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp]),
+    'yb_draw_masks': (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp]),
+    'yb_draw_cutout': (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]),
     'yb_eval_state_bytes': (C.c_size_t, [C.POINTER(EvalParams)]),
     'yb_eval_match_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.POINTER(EvalParams)]),
     'yb_eval_ap_workspace_bytes': (C.c_size_t, [C.c_int64, C.POINTER(EvalParams)]),

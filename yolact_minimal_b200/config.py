@@ -44,7 +44,8 @@ CUSTOM_CLASSES = ('dog', 'person', 'bear', 'sheep')
 norm_mean = np.array([103.94, 116.78, 123.68], dtype=np.float32)
 norm_std = np.array([57.38, 57.12, 58.40], dtype=np.float32)
 
-# Per-class drawing colours (only used by visualisation code, which is out of scope here).
+# Per-class drawing colours of utils/output_utils.draw_img (row 0: background; row id + 1: class id).  The package's own table,
+# not the reference's.
 COLORS = np.array([[0, 0, 0]] + [[(37 * i + 90) % 256, (91 * i + 30) % 256, (173 * i + 200) % 256]
                                  for i in range(80)], dtype='uint8')
 

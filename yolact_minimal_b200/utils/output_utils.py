@@ -1,10 +1,12 @@
-"""Post-process API kept from the reference's utils/output_utils.py -- `nms` (:126-163) and
-`after_nms` (:200-233) -- with the work done by the CUDA kernels behind yb_detect /
-yb_mask_assemble (include/yolact_b200.h).  Same arguments, same return tuples, same
-"(None, ...)" convention for "no detections".  `detect_batched` is the batched form the
-reference lacks (its nms() squeezes a batch of 1, output_utils.py:127-130).
+"""Post-process API kept from the reference's utils/output_utils.py -- `nms` (:126-163),
+`after_nms` (:200-233) and `draw_img` (:308-369) -- with the work done by the CUDA kernels behind
+yb_detect / yb_mask_assemble / yb_draw_masks (include/yolact_b200.h).  Same arguments, same return
+tuples, same "(None, ...)" convention for "no detections".  `detect_batched` is the batched form the
+reference lacks (its nms() squeezes a batch of 1, output_utils.py:127-130); `blend_masks` is
+draw_img's overlay on device-resident frames.
 
-All inputs must be CUDA float32 tensors; nothing here falls back to the CPU.
+All inputs must be CUDA tensors (draw_img also takes numpy arrays, which it uploads); nothing here
+falls back to the CPU.
 """
 import ctypes
 
@@ -15,6 +17,7 @@ from .box_utils import anchors_tensor
 
 _ws_cache = {}
 _anchor_cache = {}
+_palette_cache = {}
 
 
 def _params(cfg, num_classes, coef_dim, no_clip=False):
@@ -221,3 +224,150 @@ class _NoVisual:
         if k == 'visual_thre':
             return 0
         return getattr(self._cfg, k)
+
+
+# ---------------------------------------------------------------------------------------------------------------------------
+# Drawing (utils/output_utils.py:308-369).  The mask overlay and the cutout matting run on the device (csrc/draw.cu); the box,
+# label and fps pass is the reference's cv2 calls in the reference's order on the host image, which the caller needs there anyway
+# (cv2.imwrite, VideoWriter).  Colours come from config.COLORS, this package's palette.
+# ---------------------------------------------------------------------------------------------------------------------------
+def _palette(num_classes, device):
+    from ..config import COLORS
+    nc = int(num_classes) - 1
+    if not 1 <= nc <= len(COLORS):
+        raise ValueError(f'num_classes={num_classes}: the palette has {len(COLORS)} colours')
+    key = device.index
+    pal = _palette_cache.get(key)
+    if pal is None:
+        pal = torch.from_numpy(COLORS.reshape(-1).copy()).to(device)
+        _palette_cache[key] = pal
+    return pal, nc
+
+
+def _mask_operand(masks, n, h, w):
+    """masks -> (contiguous 16-byte aligned CUDA tensor, yb mask code): float32 -> 1, uint8 / bool -> 0, int32 -> 2 (packed bits
+    [n,h,ceil(w/32)], the after_nms(mask_dtype='bits') layout)."""
+    if masks.dtype == torch.int32:
+        fmt, shape = 2, (n, h, (w + 31) // 32)
+    elif masks.dtype == torch.float32:
+        fmt, shape = 1, (n, h, w)
+    elif masks.dtype in (torch.uint8, torch.bool):
+        fmt, shape = 0, (n, h, w)
+        masks = masks.view(torch.uint8)
+    else:
+        raise _lib.YolactB200Error(f'masks of dtype {masks.dtype}: expected float32, uint8, bool or int32 (packed bits)')
+    if tuple(masks.shape) != shape:
+        raise _lib.YolactB200Error(f'masks {tuple(masks.shape)} do not match {n} detections on a {h}x{w} image (expected {shape})')
+    masks = masks.contiguous()
+    return (masks if masks.data_ptr() % 16 == 0 else masks.clone()), fmt
+
+
+def _draw_operands(img, ids, masks):
+    _require_cuda(img, ids, masks)
+    if img.dtype != torch.uint8 or img.dim() != 3 or img.shape[2] != 3:
+        raise ValueError(f'img must be uint8 [h,w,3], got {img.dtype} {tuple(img.shape)}')
+    if not (ids.device == masks.device == img.device):
+        raise _lib.YolactB200Error('img, ids and masks must be on the same device')
+    h, w = int(img.shape[0]), int(img.shape[1])
+    m, fmt = _mask_operand(masks, int(ids.shape[0]), h, w)
+    return img.contiguous(), ids.to(torch.int32).contiguous(), m, fmt, h, w
+
+
+def blend_masks(img, ids, masks, num_classes):
+    """draw_img's mask overlay on device-resident frames (utils/output_utils.py:322-326): every pixel becomes
+    cv2.addWeighted(COLORS[semantic], 0.4, img, 0.6, 0) with semantic = (sum_i masks_i * (ids_i + 1)) % (num_classes - 1).
+    img CUDA uint8 [h,w,3]; ids [n] integer class ids; masks [n,h,w] {0,1} float32 / uint8 / bool, or int32 packed bits
+    [n,h,ceil(w/32)].  Returns a new CUDA uint8 [h,w,3].  One kernel launch."""
+    img, ids32, m, fmt, h, w = _draw_operands(img, ids, masks)
+    pal, nc = _palette(num_classes, img.device)
+    out = torch.empty_like(img)
+    L = _lib.lib()
+    with torch.cuda.device(img.device):
+        _lib.check(L.yb_draw_masks(img.data_ptr(), h, w, m.data_ptr(), fmt, int(ids32.shape[0]), ids32.data_ptr(), pal.data_ptr(), nc,
+                                   out.data_ptr(), torch.cuda.current_stream().cuda_stream), 'yb_draw_masks')
+    return out
+
+
+def cutout_masks(img, ids, boxes, masks, num_classes):
+    """draw_img's cfg.cutout images (utils/output_utils.py:328-341) on the device.  Returns (total_obj [h,w,3], [crop_i]) as host
+    uint8 arrays: total_obj = img where the semantic index is non-zero, else 255; crop_i = (img where masks_i, else 255)[y1:y2,
+    x1:x2] with numpy's slicing of the int box (x1, y1, x2, y2) = boxes[i] (a host array)."""
+    import numpy as np
+    img, ids32, m, fmt, h, w = _draw_operands(img, ids, masks)
+    n = int(ids32.shape[0])
+    yyxx = np.zeros((max(n, 1), 4), np.int32)
+    off = np.zeros(n + 1, np.int64)
+    for i in range(n):
+        x1, y1, x2, y2 = (int(v) for v in boxes[i, :4])
+        ya, yb, _ = slice(y1, y2).indices(h)
+        xa, xb, _ = slice(x1, x2).indices(w)
+        yyxx[i] = ya, max(ya, yb), xa, max(xa, xb)
+        off[i + 1] = off[i] + 3 * (yyxx[i, 1] - ya) * (yyxx[i, 3] - xa)
+    dev = img.device
+    total = torch.empty_like(img)
+    crops = torch.empty(max(int(off[-1]), 1), dtype=torch.uint8, device=dev)
+    yyxx_d, off_d = torch.from_numpy(yyxx).to(dev), torch.from_numpy(off).to(dev)
+    _, nc = _palette(num_classes, dev)
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        _lib.check(L.yb_draw_cutout(img.data_ptr(), h, w, m.data_ptr(), fmt, n, ids32.data_ptr(), nc, yyxx_d.data_ptr(), off_d.data_ptr(),
+                                    total.data_ptr(), crops.data_ptr(), torch.cuda.current_stream().cuda_stream), 'yb_draw_cutout')
+    flat = crops.cpu().numpy()
+    out = [flat[off[i]:off[i + 1]].reshape(yyxx[i, 1] - yyxx[i, 0], yyxx[i, 3] - yyxx[i, 2], 3) for i in range(n)]
+    return total.cpu().numpy(), out
+
+
+def draw_img(ids_p, class_p, box_p, mask_p, img_origin, cfg, img_name=None, fps=None):
+    """Reference signature (utils/output_utils.py:308).  Returns the drawn uint8 [h,w,3] image: `img_origin` itself when ids_p is
+    None, and drawn in place when cfg.hide_mask (as the reference does; cfg.real_time then returns a new array).
+    ids_p / class_p / box_p / mask_p: after_nms' CUDA tensors (masks float32, uint8, or int32 packed bits from
+    mask_dtype='bits') or numpy arrays (after_nms_numpy: bool masks), which are uploaded.  img_origin: host uint8 BGR [h,w,3],
+    uploaded once; the overlay (and the cfg.cutout matting) runs on the device, then one copy of the image comes back for the
+    box / label / fps pass, which uses the reference's cv2 calls."""
+    if ids_p is None:
+        return img_origin
+    import cv2
+    import numpy as np
+    from ..config import COLORS
+    args = (ids_p, class_p, box_p, mask_p)
+    if any(isinstance(t, torch.Tensor) and not t.is_cuda for t in args):
+        raise _lib.YolactB200Error('draw_img needs CUDA tensors or numpy arrays (no CPU fallback)')
+    if not (isinstance(img_origin, np.ndarray) and img_origin.dtype == np.uint8 and img_origin.ndim == 3 and img_origin.shape[2] == 3):
+        raise ValueError('img_origin must be a host uint8 [h,w,3] array')
+    host = lambda t: t.cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t)
+    ids_np, scores_np, boxes_np = host(ids_p), host(class_p), host(box_p)
+    img_fused = img_origin
+    if not cfg.hide_mask:
+        cuda_args = [t for t in args if isinstance(t, torch.Tensor)]
+        dev = cuda_args[0].device if cuda_args else _np_dev()
+        up = lambda t: t if isinstance(t, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(t)).to(dev)
+        ids_d, masks_d = up(ids_p), up(mask_p)
+        img_d = torch.from_numpy(np.ascontiguousarray(img_origin)).to(dev)
+        fused_d = blend_masks(img_d, ids_d, masks_d, cfg.num_classes)
+        if cfg.cutout:
+            total, crops = cutout_masks(img_d, ids_d, boxes_np, masks_d, cfg.num_classes)
+            cv2.imwrite(f'results/images/{img_name}_total_obj.jpg', total)
+            for i, crop in enumerate(crops):
+                cv2.imwrite(f'results/images/{img_name}_{i}.jpg', crop)
+        img_fused = fused_d.cpu().numpy()
+    scale = 0.6
+    thickness = 1
+    font = cv2.FONT_HERSHEY_DUPLEX
+    if not cfg.hide_bbox:
+        for i in reversed(range(ids_np.shape[0])):
+            x1, y1, x2, y2 = (int(v) for v in boxes_np[i, :])
+            color = COLORS[ids_np[i] + 1].tolist()
+            cv2.rectangle(img_fused, (x1, y1), (x2, y2), color, thickness)
+            class_name = cfg.class_names[ids_np[i]]
+            text_str = f'{class_name}: {scores_np[i]:.2f}' if not cfg.hide_score else class_name
+            text_w, text_h = cv2.getTextSize(text_str, font, scale, thickness)[0]
+            cv2.rectangle(img_fused, (x1, y1), (x1 + text_w, y1 + text_h + 5), color, -1)
+            cv2.putText(img_fused, text_str, (x1, y1 + 15), font, scale, (255, 255, 255), thickness, cv2.LINE_AA)
+    if cfg.real_time:
+        fps_str = f'fps: {fps:.2f}'
+        text_w, text_h = cv2.getTextSize(fps_str, font, scale, thickness)[0]
+        img_fused = img_fused.astype(np.float32)        # a shadow behind the fps text
+        img_fused[0:text_h + 8, 0:text_w + 8] *= 0.6
+        img_fused = img_fused.astype(np.uint8)
+        cv2.putText(img_fused, fps_str, (0, text_h + 2), font, scale, (255, 255, 255), thickness, cv2.LINE_AA)
+    return img_fused
