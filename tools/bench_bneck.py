@@ -3,10 +3,11 @@
     python tools/bench_bneck.py [--arch res101] [--size 550] [--batch 64] [--precision fp16] [--forwards 5] [--json OUT]
 
 Builds the network (synthetic weights, seeded input), runs the engine's per-op profiling pass (CUDA events around every op,
-YOLACT_B200_PROFILE_DUMP) and prints one line per k_bneck_tc launch: stage, h_out, ms, the algorithmic bytes of the pair
-(t2 / block input read, x' and t1 written once, both weights) and the rate they imply as a share of the H100 SXM data sheet's
-3.35 TB/s.  It then rebuilds the network with YOLACT_B200_NO_FUSE=1 and prints the k_conv_tc launches that replace each fused
-launch (conv3 + residual + ReLU, the next block's conv1 and, for the folded first block of layer1, the downsample convolution),
+YOLACT_B200_PROFILE_DUMP) and prints one line per k_bneck_tc launch: stage (`layer1→2` / `layer2→3` for the launches that end
+a stage and feed the next stage's first conv1), h_out, ms, the algorithmic bytes of the pair (t2 / block input read, x' and t1
+written once, both weights) and the rate they imply as a share of the H100 SXM data sheet's 3.35 TB/s.  It then rebuilds the
+network with YOLACT_B200_NO_FUSE=1 and prints the k_conv_tc launches that replace each fused launch (conv3 + residual + ReLU,
+the next block's conv1 and, for the folded first block of layer1, the downsample convolution),
 so the unfused path is the control measured on the same card in the same run.  The card's name, power limit and max SM clock
 are read in the same run."""
 import argparse
@@ -23,6 +24,8 @@ if ROOT not in sys.path:
 
 HBM_GBS = 3350.0            # NVIDIA H100 SXM data sheet (700 W)
 OP_CONV, OP_BNECK = 3, 11   # net.cu OpKind
+# (Cin, Cexp, Cout) widths k_bneck_tc fuses (conv_tc.cu bneck_supported): within a stage, and into the next stage's first conv1
+FUSED_WIDTHS = {(64, 256, 64), (128, 512, 128), (256, 1024, 256), (64, 256, 128), (128, 512, 256)}
 
 
 def card():
@@ -98,12 +101,12 @@ def main():
     fused = [o for o in profile_rows(args.arch, args.size, args.batch, args.precision, args.forwards, True) if o['kind'] == OP_BNECK]
     plain = profile_rows(args.arch, args.size, args.batch, args.precision, args.forwards, False)
 
-    # the unfused launches of each fused one, in network order: [downsample] conv3 (Cmid -> Cexp) conv1 (Cexp -> Cmid)
+    # the unfused launches of each fused one, in network order: [downsample] conv3 (Cin -> Cexp, + residual) conv1 (Cexp -> Cout)
     groups = []
     for j in range(len(plain) - 1):
         a, b = plain[j], plain[j + 1]
-        if (a['kind'] == b['kind'] == OP_CONV and a['k'] == b['k'] == 1 and a['cout'] == 4 * a['cin'] == b['cin'] and b['cout'] == a['cin']
-                and a['h_out'] == b['h_out'] and a['cin'] in (64, 128, 256)):
+        if (a['kind'] == b['kind'] == OP_CONV and a['k'] == b['k'] == 1 and a['stride'] == b['stride'] == 1 and a['res'] == 1
+                and a['cout'] == b['cin'] and a['h_out'] == b['h_out'] and (a['cin'], a['cout'], b['cout']) in FUSED_WIDTHS):
             g = [a, b]
             d = plain[j - 1]
             if d['kind'] == OP_CONV and d['k'] == 1 and d['cout'] == a['cout'] and d['h_out'] == a['h_out']:
@@ -112,24 +115,27 @@ def main():
     assert len(groups) == len(fused), f'{len(fused)} fused launches but {len(groups)} unfused pairs'
 
     esz = 2
-    stages = {h: f'layer{i + 1}' for i, h in enumerate(sorted({o['h_out'] for o in fused}, reverse=True))}
+    layer = {h: i + 1 for i, h in enumerate(sorted({o['h_out'] for o in fused}, reverse=True))}
     print(json.dumps(dict(info, arch=args.arch, size=args.size, batch=args.batch, precision=args.precision, forwards=args.forwards)))
-    print(f'{"#":>3} {"stage":7} {"h_out":>5} {"Cmid":>4} {"fold":>4} {"fused ms":>9} {"MB":>7} {"GB/s":>7} {"%HBM":>5} {"unfused ms":>10} {"fused/unfused":>13}')
+    print(f'{"#":>3} {"stage":8} {"h_out":>5} {"Cin":>4} {"Cout":>4} {"fold":>4} {"fused ms":>9} {"MB":>7} {"GB/s":>7} {"%HBM":>5} {"unfused ms":>10} '
+          f'{"fused/unfused":>13}')
     launches, tot_f, tot_u, tot_b = [], 0.0, 0.0, 0.0
     for n, (f, g) in enumerate(zip(fused, groups)):
-        cmid, cexp, px = f['cin'], f['cout'], float(args.batch) * f['h_out'] ** 2
+        cin, cexp, cout, px = f['cin'], f['cout'], g[-1]['cout'], float(args.batch) * f['h_out'] ** 2
+        assert (g[-2]['cin'], g[-2]['cout'], g[-2]['h_out']) == (cin, cexp, f['h_out']), (f, g)
+        stage = f'layer{layer[f["h_out"]]}' + (f'→{layer[f["h_out"]] + 1}' if cout != cin else '')
         fold = len(g) == 3
-        nbytes = px * esz * (2.0 * cmid + 2.0 * cexp) + 2.0 * cexp * cmid * esz           # net.cu yb_net_profile's formula
+        nbytes = px * esz * (cin + 2.0 * cexp + cout) + cexp * (cin + cout) * esz           # net.cu yb_net_profile's formula
         if fold:
             cd = g[0]['cin']
             nbytes += px * esz * (cd - cexp) + cexp * cd * esz
         ms_u = sum(o['ms'] for o in g)
         gbs = nbytes / (f['ms'] * 1e-3) / 1e9
-        rec = {'launch': n, 'stage': stages[f['h_out']], 'h_out': f['h_out'], 'Cmid': cmid, 'folded_downsample': fold, 'ms': f['ms'],
+        rec = {'launch': n, 'stage': stage, 'h_out': f['h_out'], 'Cin': cin, 'Cout': cout, 'folded_downsample': fold, 'ms': f['ms'],
                'bytes': nbytes, 'gbs': gbs, 'hbm_frac': gbs / HBM_GBS, 'unfused_ms': ms_u, 'unfused_launches': [o['ms'] for o in g]}
         launches.append(rec)
         tot_f += f['ms']; tot_u += ms_u; tot_b += nbytes
-        print(f'{n:3d} {rec["stage"]:7} {f["h_out"]:5d} {cmid:4d} {"yes" if fold else "":>4} {f["ms"]:9.4f} {nbytes / 1e6:7.1f} {gbs:7.0f} '
+        print(f'{n:3d} {stage:8} {f["h_out"]:5d} {cin:4d} {cout:4d} {"yes" if fold else "":>4} {f["ms"]:9.4f} {nbytes / 1e6:7.1f} {gbs:7.0f} '
               f'{100 * gbs / HBM_GBS:4.1f}% {ms_u:10.4f} {f["ms"] / ms_u:13.3f}')
     per_stage = {}
     for r in launches:

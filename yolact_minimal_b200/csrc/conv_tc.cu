@@ -483,13 +483,15 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 // =================================================================================================================
 // Fused bottleneck tail + next head (layers.cuh BneckArgs), persistent, one 128-row tile at a time, the same three warpgroups:
 //   for each 128-channel chunk c of the expanded width:
-//     A(c):  accA  = t2 * W3_c^T                 (wgmma m64n128, K = Cmid [+ Cd: the folded downsample branch])
+//     A(c):  accA  = t2 * W3_c^T                 (wgmma m64n128, K = Cin [+ Cd: the folded downsample branch])
 //     E(c):  x'_c  = relu(accA + b3_c [+ x_c])   -> 16 bit, in shared memory in the 128B-swizzled A-operand layout -> xo (TMA store)
-//     B(c):  accB += x'_c * W1_c^T               (wgmma m64nCmid, K = 128)
+//     B(c):  accB += x'_c * W1_c^T               (wgmma m64nCout, K = 128)
 //   t1 = relu(accB + b1) -> HBM.
+// Cin is the t2 width (this block's conv3 input), Cout the t1 width (the next block's conv1 output): equal inside a stage, Cout =
+// 2 Cin where the next block opens a stage (layer1 -> layer2: 64 -> 256 -> 128, layer2 -> layer3: 128 -> 512 -> 256).
 // x' never makes a round trip through HBM before the next block's conv1.  The operand rounding points, the k order and the epilogue
 // arithmetic are those of the two separate k_conv_tc launches, so the result is bit-identical to the unfused pair (the folded
-// downsample branch skips one 16-bit rounding of the residual).  Both GEMMs' accumulators live in registers (64 + Cmid / 2 per
+// downsample branch skips one 16-bit rounding of the residual).  Both GEMMs' accumulators live in registers (64 + Cout / 2 per
 // thread), so the consumers take 232 registers from the producer with setmaxnreg.
 //
 // Shared memory: the t2 tile (resident for the whole tile), two x buffers and a ring of weight slots in the order the consumers use
@@ -497,13 +499,14 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
 // into it by TMA one chunk ahead; E(c) reads x_c and writes x'_c at the same swizzled address, so the buffer is in turn the residual,
 // the A operand of B(c) and the source of the TMA store of xo (rows >= M are clipped by the store's tensor map).  A buffer is handed
 // back to the producer once B(c) has retired and the store has read it.  Both GEMMs keep one k-block in flight and release a slot
-// when it retires; B(c)'s last k-block retires under A(c+1).  At Cmid = 256 one 32 KiB slot holds either two W3 k-blocks or one
-// W1 k-block.
+// when it retires; B(c)'s last k-block retires under A(c+1).  Every slot is 16 KiB: one W3 k-block [128 rows][128 B], or one 128-row
+// part of a W1 k-block ([min(Cout, 128) rows][128 B]; at Cout = 256 a W1 k-block is two parts, each the B operand of an m64n128 wgmma
+// into its half of accB).  Small slots release early: a consumer warpgroup holds two (the group in flight and the one it issues),
+// and the rest of the ring is the producer's lookahead.
 // =================================================================================================================
 struct BnParams {
   long long M;
   int m_tiles, Cexp, nch, kbA, kbT, has_res, slots;
-  uint32_t slot_bytes;
   Geom g;
   const float* b3;
   const float* b1;
@@ -511,19 +514,21 @@ struct BnParams {
 };
 
 constexpr uint32_t BN_X_BYTES = 2 * TC_A_STAGE;                  // one x buffer: 128 rows x 128 channels
+constexpr uint32_t BN_SLOT = TC_A_STAGE;                         // one ring slot: 128 rows x 128 B
 
-template <bool F16, int CMID>
+template <bool F16, int COUT>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUtensorMap tmXd, const __grid_constant__ CUtensorMap tmW3,
            const __grid_constant__ CUtensorMap tmW1, const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmXo,
            const BnParams p) {
-  constexpr int WPS = CMID == 256 ? 2 : 1;                       // W3 k-blocks per ring slot
+  constexpr int W1R = COUT < 128 ? COUT : 128;                   // rows of one W1 part (one ring slot)
+  constexpr int W1P = COUT / W1R;                                // W1 parts per k-block
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* sT2 = smem;                                         // [kbA][128 rows x 128 B]
   uint8_t* sX = sT2 + (size_t)p.kbA * TC_A_STAGE;              // [2 buffers][2 k-blocks][128 rows x 128 B]
-  uint8_t* sRing = sX + 2 * BN_X_BYTES;                        // [slots][slot_bytes]
-  uint64_t* full = reinterpret_cast<uint64_t*>(sRing + (size_t)p.slots * p.slot_bytes);
+  uint8_t* sRing = sX + 2 * BN_X_BYTES;                        // [slots][BN_SLOT]
+  uint64_t* full = reinterpret_cast<uint64_t*>(sRing + (size_t)p.slots * BN_SLOT);
   uint64_t* empty = full + TC_MAX_STAGES;
   uint64_t* t2_full = empty + TC_MAX_STAGES;
   uint64_t* t2_empty = t2_full + 1;
@@ -563,18 +568,16 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
           } else {
             mbar_arrive(&x_full[xb]);                               // folded branch: no residual, the buffer only holds x'
           }
-          for (int kb = 0; kb < p.kbA; kb += WPS) {                 // W3 rows c*128 .., k-blocks kb .. kb + WPS - 1
+          for (int kb = 0; kb < p.kbA; ++kb) {                      // W3 rows c*128 .., k-block kb
             mbar_wait(&empty[stage], phase ^ 1);
-            mbar_expect_tx(&full[stage], WPS * TC_A_STAGE);
-#pragma unroll
-            for (int w = 0; w < WPS; ++w)
-              tma_load_2d(sRing + (size_t)stage * p.slot_bytes + (size_t)w * TC_A_STAGE, &tmW3, (kb + w) * TC_BK, c * 128, &full[stage]);
+            mbar_expect_tx(&full[stage], TC_A_STAGE);
+            tma_load_2d(sRing + (size_t)stage * BN_SLOT, &tmW3, kb * TC_BK, c * 128, &full[stage]);
             if (++stage == p.slots) { stage = 0; phase ^= 1; }
           }
-          for (int kb = 0; kb < 2; ++kb) {                          // W1[:, c*128 + kb*64 ..]: all CMID rows
+          for (int kb = 0; kb < 2 * W1P; ++kb) {                    // W1[part * W1R .., c*128 + (kb / W1P)*64 ..]
             mbar_wait(&empty[stage], phase ^ 1);
-            mbar_expect_tx(&full[stage], (uint32_t)CMID * 128u);
-            tma_load_2d(sRing + (size_t)stage * p.slot_bytes, &tmW1, c * 128 + kb * TC_BK, 0, &full[stage]);
+            mbar_expect_tx(&full[stage], (uint32_t)W1R * 128u);
+            tma_load_2d(sRing + (size_t)stage * BN_SLOT, &tmW1, c * 128 + (kb / W1P) * TC_BK, (kb % W1P) * W1R, &full[stage]);
             if (++stage == p.slots) { stage = 0; phase ^= 1; }
           }
         }
@@ -588,7 +591,7 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
     const bool signal = lane == 0;
     griddep_wait();
     float accA[64];
-    float accB[CMID / 2];
+    float accB[COUT / 2];
     int stage = 0; uint32_t phase = 0;
     int prev = -1;                                               // ring slot whose MMAs are still in flight
     int xpend = -1;                                              // x buffer read by the in-flight B(c)
@@ -616,19 +619,15 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
       for (int c = 0; c < p.nch; ++c, ++q) {
         const int xb = q & 1;
         // ---- A(c) ----
-        for (int kb = 0; kb < p.kbA; kb += WPS) {
+        for (int kb = 0; kb < p.kbA; ++kb) {
           mbar_wait(&full[stage], phase);
-          const uint32_t slot = smem_u32(sRing + (size_t)stage * p.slot_bytes);
+          const uint64_t da = gmma_desc(smem_u32(sT2 + (size_t)kb * TC_A_STAGE + (size_t)cw * (TC_A_STAGE / 2)));
+          const uint64_t db = gmma_desc(smem_u32(sRing + (size_t)stage * BN_SLOT));
           acc_fence<64>(accA);
           wgmma_fence();
 #pragma unroll
-          for (int w = 0; w < WPS; ++w) {
-            const uint64_t da = gmma_desc(smem_u32(sT2 + (size_t)(kb + w) * TC_A_STAGE + (size_t)cw * (TC_A_STAGE / 2)));
-            const uint64_t db = gmma_desc(slot + (uint32_t)w * TC_A_STAGE);
-#pragma unroll
-            for (int k = 0; k < TC_BK / 16; ++k)
-              wgmma_n128<F16, 0>(accA, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), ((kb + w) | k) != 0 ? 1u : 0u);
-          }
+          for (int k = 0; k < TC_BK / 16; ++k)
+            wgmma_n128<F16, 0>(accA, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (kb | k) != 0 ? 1u : 0u);
           wgmma_commit();
           wgmma_wait<1>();                                         // the previous group (a W3 slot, or B(c-1)'s last k-block) has retired
           acc_fence<64>(accA);
@@ -672,19 +671,20 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
             tma_store_2d(&tmXo, sX + (size_t)xb * BN_X_BYTES + (size_t)kb * TC_A_STAGE + (size_t)cw * (TC_A_STAGE / 2), c * 128 + kb * TC_BK, row);
           bulk_commit();
         }
-        // ---- B(c) ----
-        for (int kb = 0; kb < 2; ++kb) {
+        // ---- B(c): k-block kb / W1P, W1 part kb % W1P -> columns (kb % W1P) * W1R .. of accB ----
+#pragma unroll
+        for (int kb = 0; kb < 2 * W1P; ++kb) {
           mbar_wait(&full[stage], phase);
-          const uint64_t da = gmma_desc(sXw + (uint32_t)kb * TC_A_STAGE);
-          const uint64_t db = gmma_desc(smem_u32(sRing + (size_t)stage * p.slot_bytes));
-          acc_fence<CMID / 2>(accB);
+          const uint64_t da = gmma_desc(sXw + (uint32_t)(kb / W1P) * TC_A_STAGE);
+          const uint64_t db = gmma_desc(smem_u32(sRing + (size_t)stage * BN_SLOT));
+          acc_fence<COUT / 2>(accB);
           wgmma_fence();
 #pragma unroll
           for (int k = 0; k < TC_BK / 16; ++k)
-            wgmma_tile<CMID, F16, 0>(accB, da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | kb | k) != 0 ? 1u : 0u);
+            wgmma_tile<W1R, F16, 0>(accB + (kb % W1P) * (W1R / 2), da + (uint64_t)(k * 2), db + (uint64_t)(k * 2), (c | (kb / W1P) | k) != 0 ? 1u : 0u);
           wgmma_commit();
           wgmma_wait<1>();
-          acc_fence<CMID / 2>(accB);
+          acc_fence<COUT / 2>(accB);
           if (prev >= 0) release(prev);
           prev = stage;
           if (++stage == p.slots) { stage = 0; phase ^= 1; }
@@ -692,23 +692,27 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
         xpend = xb;
       }
       wgmma_wait<0>();
-      acc_fence<CMID / 2>(accB);
+      acc_fence<COUT / 2>(accB);
       release(prev);
       prev = -1;
       release_x(xpend);
       xpend = -1;
       // ---- t1 = relu(accB + b1), halo rows zero ----
+      // Lane l of a quad holds 4 bytes of a row per column group j (words 4j + l).  One xor shuffle between lanes l and l ^ 1 gives
+      // each lane 8 contiguous bytes of group 2g (even lanes) or 2g + 1 (odd lanes), so a quad stores a full 32-byte sector per row.
       const float2* b1 = reinterpret_cast<const float2*>(p.b1) + (lane & 3);
-      uint32_t* t1row[2];
+      const bool odd = lane & 1;
 #pragma unroll
-      for (int h = 0; h < 2; ++h) t1row[h] = reinterpret_cast<uint32_t*>((uint16_t*)p.t1 + m[h] * CMID) + (lane & 3);
-#pragma unroll
-      for (int j = 0; j < CMID / 8; ++j) {
-        const float2 b = __ldg(b1 + 4 * j);
+      for (int g = 0; g < COUT / 16; ++g) {
+        const float2 ba = __ldg(b1 + 8 * g), bb = __ldg(b1 + 8 * g + 4);         // groups 2g, 2g + 1: shared by both rows
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          const uint32_t pk = pack2<F16>(apply_act(b.x + accB[4 * j + 2 * h], 1), apply_act(b.y + accB[4 * j + 2 * h + 1], 1));
-          if (valid[h]) t1row[h][4 * j] = zero[h] ? 0u : pk;
+          uint32_t v0 = pack2<F16>(apply_act(ba.x + accB[8 * g + 2 * h], 1), apply_act(ba.y + accB[8 * g + 2 * h + 1], 1));
+          uint32_t v1 = pack2<F16>(apply_act(bb.x + accB[8 * g + 4 + 2 * h], 1), apply_act(bb.y + accB[8 * g + 4 + 2 * h + 1], 1));
+          const uint32_t r = __shfl_xor_sync(0xffffffffu, odd ? v0 : v1, 1);
+          if (odd) v0 = r; else v1 = r;
+          if (valid[h])
+            reinterpret_cast<uint2*>((uint16_t*)p.t1 + m[h] * COUT)[4 * g + 2 * (lane & 1) + ((lane >> 1) & 1)] = zero[h] ? make_uint2(0u, 0u) : make_uint2(v0, v1);
         }
       }
     }
@@ -959,13 +963,12 @@ int launch_conv_tc(const TcPlan* pl, const ConvArgs& a, cudaStream_t s) {
 // ---- fused bottleneck tail (k_bneck_tc) ------------------------------------------------------------------------------
 struct BnPlan {
   CUtensorMap tmT2, tmXd, tmW3, tmW1, tmX;                         // tmX: the residual, read by TMA in 128-row boxes
-  int sms, Cmid, Cd, slots;
-  uint32_t slot_bytes;
+  int sms, Cin, Cout, Cd, slots;
   size_t smem_bytes;
 };
 
-template <class F> static cudaError_t with_bneck_kernel(bool f16, int cmid, F&& f) {
-  switch (cmid) {
+template <class F> static cudaError_t with_bneck_kernel(bool f16, int cout, F&& f) {
+  switch (cout) {
     case 64: return f16 ? f(k_bneck_tc<true, 64>) : f(k_bneck_tc<false, 64>);
     case 128: return f16 ? f(k_bneck_tc<true, 128>) : f(k_bneck_tc<false, 128>);
     case 256: return f16 ? f(k_bneck_tc<true, 256>) : f(k_bneck_tc<false, 256>);
@@ -973,36 +976,39 @@ template <class F> static cudaError_t with_bneck_kernel(bool f16, int cmid, F&& 
   return cudaErrorInvalidValue;
 }
 
-bool bneck_supported(int act_dt, int Cmid, int Cexp) {
-  return (act_dt == DT_F16 || act_dt == DT_BF16) && (Cmid == 64 || Cmid == 128 || Cmid == 256) && Cexp == 4 * Cmid && !getenv("YOLACT_B200_NO_FUSE");
+// (Cin, Cexp, Cout): the stride-1 blocks of layer1 / layer2 / layer3 (Cout = Cin) and the first blocks of layer2 / layer3 (Cout = 2 Cin).
+// Not layer3 -> layer4 (256, 1024, 512): accB would need 256 registers per thread.
+bool bneck_supported(int act_dt, int Cin, int Cexp, int Cout) {
+  const bool widths = Cexp == 4 * Cin && (((Cin == 64 || Cin == 128 || Cin == 256) && Cout == Cin) || ((Cin == 64 || Cin == 128) && Cout == 2 * Cin));
+  return (act_dt == DT_F16 || act_dt == DT_BF16) && widths && !getenv("YOLACT_B200_NO_FUSE");
 }
 
 int bneck_plan_create(const BneckArgs& a, int max_batch, BnPlan** out) {
-  YB_REQUIRE(bneck_supported(a.act_dt, a.Cmid, a.Cexp), YB_ERR_UNSUPPORTED, "bneck_plan_create: unsupported Cmid=%d Cexp=%d", a.Cmid, a.Cexp);
-  YB_REQUIRE(a.Cd == 0 || (a.xd && a.Cd % 64 == 0 && (a.Cmid + a.Cd) / 64 <= 4), YB_ERR_UNSUPPORTED, "bneck_plan_create: folded residual branch with Cd=%d", a.Cd);
+  YB_REQUIRE(bneck_supported(a.act_dt, a.Cin, a.Cexp, a.Cout), YB_ERR_UNSUPPORTED, "bneck_plan_create: unsupported Cin=%d Cexp=%d Cout=%d", a.Cin,
+             a.Cexp, a.Cout);
+  YB_REQUIRE(a.Cd == 0 || (a.xd && a.Cd % 64 == 0 && (a.Cin + a.Cd) / 64 <= 4), YB_ERR_UNSUPPORTED, "bneck_plan_create: folded residual branch with Cd=%d", a.Cd);
   YB_REQUIRE(a.Cd != 0 || a.x, YB_ERR_INVALID, "bneck_plan_create: no residual");
   BnPlan* pl = new BnPlan();
-  pl->Cmid = a.Cmid; pl->Cd = a.Cd;
-  const int kbA = (a.Cmid + a.Cd) / 64;
-  pl->slot_bytes = (uint32_t)(a.Cmid * 128 > (int)TC_A_STAGE ? a.Cmid * 128 : (int)TC_A_STAGE);
+  pl->Cin = a.Cin; pl->Cout = a.Cout; pl->Cd = a.Cd;
+  const int kbA = (a.Cin + a.Cd) / 64;
   const size_t fixed = 1024 /*align*/ + (2 * TC_MAX_STAGES + 6) * 8 /*barriers*/ + (size_t)kbA * TC_A_STAGE + 2 * BN_X_BYTES;
-  int slots = (int)((TC_SMEM_MAX - fixed) / pl->slot_bytes);
+  int slots = (int)((TC_SMEM_MAX - fixed) / BN_SLOT);
   pl->slots = slots > TC_MAX_STAGES ? TC_MAX_STAGES : slots;
-  pl->smem_bytes = fixed + (size_t)pl->slots * pl->slot_bytes;
+  pl->smem_bytes = fixed + (size_t)pl->slots * BN_SLOT;
   const bool f16 = a.act_dt == DT_F16;
   const uint64_t rows = (uint64_t)max_batch * a.g.plane();
   int s = pl->slots >= 2 ? YB_OK : YB_ERR_UNSUPPORTED;
-  if (s == YB_OK) s = make_map(&pl->tmT2, a.t2, (uint64_t)a.Cmid, rows, TC_BM, f16);
+  if (s == YB_OK) s = make_map(&pl->tmT2, a.t2, (uint64_t)a.Cin, rows, TC_BM, f16);
   pl->tmXd = pl->tmT2;                                             // placeholder without a folded branch
   if (s == YB_OK && a.Cd) s = make_map(&pl->tmXd, a.xd, (uint64_t)a.Cd, rows, TC_BM, f16);
   pl->tmX = pl->tmT2;                                              // placeholder with a folded branch (no residual read)
   if (s == YB_OK && !a.Cd) s = make_map(&pl->tmX, a.x, (uint64_t)a.Cexp, rows, TC_BM, f16);
-  if (s == YB_OK) s = make_map(&pl->tmW3, a.w3, (uint64_t)(a.Cmid + a.Cd), (uint64_t)a.Cexp, 128, f16);
-  if (s == YB_OK) s = make_map(&pl->tmW1, a.w1, (uint64_t)a.Cexp, (uint64_t)a.Cmid, (uint32_t)a.Cmid, f16);
+  if (s == YB_OK) s = make_map(&pl->tmW3, a.w3, (uint64_t)(a.Cin + a.Cd), (uint64_t)a.Cexp, 128, f16);
+  if (s == YB_OK) s = make_map(&pl->tmW1, a.w1, (uint64_t)a.Cexp, (uint64_t)a.Cout, (uint32_t)(a.Cout < 128 ? a.Cout : 128), f16);
   int dev = 0;
   if (s == YB_OK && cudaGetDevice(&dev) != cudaSuccess) s = YB_ERR_CUDA;
   if (s == YB_OK && cudaDeviceGetAttribute(&pl->sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) s = YB_ERR_CUDA;
-  if (s == YB_OK && with_bneck_kernel(f16, a.Cmid, [&](auto k) {
+  if (s == YB_OK && with_bneck_kernel(f16, a.Cout, [&](auto k) {
         return cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TC_SMEM_MAX); }) != cudaSuccess) s = YB_ERR_CUDA;
   if (s != YB_OK) { delete pl; return s; }
   *out = pl;
@@ -1016,8 +1022,8 @@ int launch_bneck_tc(const BnPlan* pl, const BneckArgs& a, cudaStream_t s) {
   memset(&p, 0, sizeof(p));
   p.M = (long long)a.B * a.g.plane();
   p.m_tiles = (int)((p.M + TC_BM - 1) / TC_BM);
-  p.Cexp = a.Cexp; p.nch = a.Cexp / 128; p.kbT = a.Cmid / 64; p.kbA = (a.Cmid + pl->Cd) / 64; p.has_res = pl->Cd ? 0 : 1;
-  p.slots = pl->slots; p.slot_bytes = pl->slot_bytes;
+  p.Cexp = a.Cexp; p.nch = a.Cexp / 128; p.kbT = pl->Cin / 64; p.kbA = (pl->Cin + pl->Cd) / 64; p.has_res = pl->Cd ? 0 : 1;
+  p.slots = pl->slots;
   p.g = a.g; p.b3 = a.b3; p.b1 = a.b1; p.t1 = a.t1;
   // xo is written by TMA stores of [64 rows x 64 channels]; the map ends at this launch's last row, so rows >= M stay untouched
   CUtensorMap tmXo;
@@ -1030,7 +1036,7 @@ int launch_bneck_tc(const BnPlan* pl, const BneckArgs& a, cudaStream_t s) {
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-  YB_CHECK_CUDA(with_bneck_kernel(a.act_dt == DT_F16, pl->Cmid, [&](auto k) { return cudaLaunchKernelEx(&cfg, k, pl->tmT2, pl->tmXd, pl->tmW3, pl->tmW1, pl->tmX, tmXo, p); }));
+  YB_CHECK_CUDA(with_bneck_kernel(a.act_dt == DT_F16, pl->Cout, [&](auto k) { return cudaLaunchKernelEx(&cfg, k, pl->tmT2, pl->tmXd, pl->tmW3, pl->tmW1, pl->tmX, tmXo, p); }));
   YB_CHECK_LAUNCH();
   return YB_OK;
 }

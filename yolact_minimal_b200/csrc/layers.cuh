@@ -78,22 +78,24 @@ struct GemmArgs {
 int tc_plan_create_gemm(const GemmArgs& g, TcPlan** out);
 int launch_gemm_tc(const TcPlan* p, const GemmArgs& g, cudaStream_t s);
 
-// Fused tail of one ResNet bottleneck and head of the next (modules/resnet.py:20-40, stride-1 blocks of one stage):
-//   xo = relu(W3 * t2 + b3 + x)            1x1 Cmid -> Cexp, residual x, written out (the next block's residual / the stage output)
-//   t1 = relu(W1 * xo + b1)                1x1 Cexp -> Cmid of the NEXT block, fed from shared memory: xo is never re-read from HBM
+// Fused tail of one ResNet bottleneck and head of the next (modules/resnet.py:20-40):
+//   xo = relu(W3 * t2 + b3 + x)            1x1 Cin -> Cexp, residual x, written out (the next block's residual / the stage output)
+//   t1 = relu(W1 * xo + b1)                1x1 Cexp -> Cout of the NEXT block, fed from shared memory: xo is never re-read from HBM
+// Cout = Cin between the stride-1 blocks of a stage; Cout = 2 Cin when the next block opens the next stage (its conv1 runs at this
+// block's resolution, its stride-2 conv2 and downsample read xo / t1 from HBM).
 // All four tensors are haloed NHWC with the same geometry; weights are the packed K-major matrices of the two convolutions.
 // First block of a stage (Cd > 0): the residual branch is itself a 1x1 convolution of the block input xd (Cd channels, same geometry);
-// it is folded into the first GEMM -- w3 is then [Cexp][Cmid + Cd] (conv3 | downsample weights side by side), b3 the summed biases, x unused.
+// it is folded into the first GEMM -- w3 is then [Cexp][Cin + Cd] (conv3 | downsample weights side by side), b3 the summed biases, x unused.
 struct BneckArgs {
   const void* t2; const void* x; const void* w3; const void* w1;
   const void* xd; int Cd;
   const float* b3; const float* b1;
   void* xo; void* t1;
-  int act_dt, B, Cmid, Cexp;
+  int act_dt, B, Cin, Cexp, Cout;
   Geom g;
 };
 struct BnPlan;
-bool bneck_supported(int act_dt, int Cmid, int Cexp);
+bool bneck_supported(int act_dt, int Cin, int Cexp, int Cout);
 int bneck_plan_create(const BneckArgs& a_maxbatch, int max_batch, BnPlan** out);
 void bneck_plan_destroy(BnPlan* p);
 int launch_bneck_tc(const BnPlan* p, const BneckArgs& a, cudaStream_t s);

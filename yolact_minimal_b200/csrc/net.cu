@@ -350,8 +350,9 @@ void build_program(yb_net* net) {
   }
 }
 
-// 16-bit modes: merge [1x1 Cmid->Cexp + residual + ReLU] followed by [1x1 Cexp->Cmid + ReLU] (conv3 of a bottleneck and conv1 of the
-// next, modules/resnet.py:20-40) into one OP_BNECK where k_bneck_tc supports the widths (layer3: 256 / 1024)
+// 16-bit modes: merge [1x1 Cin->Cexp + residual + ReLU] followed by [1x1 Cexp->Cout + ReLU] (conv3 of a bottleneck and conv1 of the
+// next, modules/resnet.py:20-40) into one OP_BNECK where k_bneck_tc supports the widths (bneck_supported: within layer1 / 2 / 3, and
+// layer1 -> layer2 / layer2 -> layer3, where the next block's conv1 still runs at this resolution)
 void fuse_bottlenecks(yb_net* net) {
   if (net->act_dt == DT_F32 || getenv("YOLACT_B200_NO_TC")) return;
   std::vector<Op> merged;
@@ -363,8 +364,8 @@ void fuse_bottlenecks(yb_net* net) {
       const ConvW& cb = net->convs[b.conv];
       const bool ok = ca.k == 1 && cb.k == 1 && a.stride == 1 && b.stride == 1 && a.res >= 0 && b.res < 0 && a.relu == 1 && b.relu == 1 &&
                       a.out_mode == 0 && b.out_mode == 0 && a.ext == EXT_NONE && b.ext == EXT_NONE && b.in == a.out && ca.cat.empty() &&
-                      cb.cat.empty() && ca.Cout == cb.Cin && cb.Cout == ca.Cin && ca.Cin == ca.Cin_pad && cb.Cin == cb.Cin_pad &&
-                      ca.Cout == ca.Cout_pad && cb.Cout == cb.Cout_pad && bneck_supported(net->act_dt, ca.Cin, ca.Cout);
+                      cb.cat.empty() && ca.Cout == cb.Cin && ca.Cin == ca.Cin_pad && cb.Cin == cb.Cin_pad && ca.Cout == ca.Cout_pad &&
+                      cb.Cout == cb.Cout_pad && bneck_supported(net->act_dt, ca.Cin, ca.Cout, cb.Cout);
       if (ok) {
         Op f = a;
         f.kind = OP_BNECK; f.conv2 = b.conv; f.out2 = b.out;
@@ -405,7 +406,7 @@ void bneck_args(const yb_net* net, const Op& o, int B, BneckArgs* a) {
   else a->x = net->slots[net->acts[o.res].slot];
   a->xo = net->slots[net->acts[o.out].slot]; a->t1 = net->slots[net->acts[o.out2].slot];
   a->w3 = o.convd >= 0 ? o.d_wcat : c3.d_w; a->b3 = o.convd >= 0 ? o.d_bcat : c3.d_b; a->w1 = c1.d_w; a->b1 = c1.d_b;
-  a->act_dt = net->act_dt; a->B = B; a->Cmid = c3.Cin; a->Cexp = c3.Cout;
+  a->act_dt = net->act_dt; a->B = B; a->Cin = c3.Cin; a->Cexp = c3.Cout; a->Cout = c1.Cout;
   a->g.H = net->acts[o.in].H; a->g.W = a->g.H;
 }
 
@@ -868,10 +869,11 @@ extern "C" int yb_net_profile(yb_net* net, yb_prof_entry* out, int max_entries, 
         }
         case OP_BNECK: {                                               // both convolutions; x' written once and never re-read
           const ConvW& c3 = net->convs[o.conv];
+          const double Cin = c3.Cin, Cexp = c3.Cout, Cout = net->convs[o.conv2].Cout;
           const double Ho = net->acts[o.in].H, px = B * Ho * Ho;
           k = 12;
-          flops = 4.0 * px * c3.Cout * c3.Cin;
-          bytes = px * esz * (2.0 * c3.Cin + 2.0 * c3.Cout) + 2.0 * c3.Cout * c3.Cin * esz;
+          flops = 2.0 * px * Cexp * (Cin + Cout);
+          bytes = px * esz * (Cin + 2.0 * Cexp + Cout) + Cexp * (Cin + Cout) * esz;   // t2, x read; x', t1 written; W3, W1
           if (o.convd >= 0) {                                          // + the folded downsample conv; its output / the residual read do not exist
             const double Cd = net->convs[o.convd].Cin;
             flops += 2.0 * px * c3.Cout * Cd;
