@@ -67,7 +67,8 @@ def test_native_losses_random_subset_when_many_positives(cuda):
     assert (nz(a) <= cfg.masks_to_train).all() and nz(a).max() == cfg.masks_to_train         # exactly masks_to_train masks get a gradient
 
 
-@pytest.mark.parametrize('arch,S,B,precision', [('res50', 128, 2, 'bf16'), ('res50', 128, 2, 'fp16'), ('res101', 96, 2, 'bf16')])
+@pytest.mark.parametrize('arch,S,B,precision', [('res50', 128, 2, 'bf16'), ('res50', 128, 2, 'fp16'), ('res101', 96, 2, 'bf16'),
+                                                ('res101', 550, 2, 'bf16')])
 def test_training_engine_backward_at_its_own_activations(cuda, arch, S, B, precision):
     """The strict check of the BACKWARD pass: the torch-autograd checker is evaluated AT the engine's stored activations (every conv
     output, BN / ReLU output, FPN level ...: identical ReLU masks and batch statistics), so that what is compared is the engine's
@@ -83,7 +84,7 @@ def test_training_engine_backward_at_its_own_activations(cuda, arch, S, B, preci
     print(f'{arch}@{S} {precision}: worst parameter gradients (rel err, cosine, |ref|):', worst, 'launches/step', o['launches'])
     tol_max, tol_med = (0.15, 3e-2) if precision == 'bf16' else (2e-2, 4e-3)
     for n, (r, c, nr) in rels.items():
-        assert r < tol_max and c > 0.99, (n, r, c, nr)                                             # EVERY parameter of the network
+        assert r < tol_max and (c > 0.99 or r == 0), (n, r, c, nr)          # EVERY parameter (r == 0: both exactly zero, no loss reaches it)
     assert float(np.median([v[0] for v in rels.values()])) < tol_med
     for name, e in o['gact'].items():
         if name not in ('c3', 'c4', 'c5'):                     # (the checker's c3..c5 taps sit on the FPN branch only in this mode)

@@ -410,14 +410,14 @@ int op_bn(yb_train* t, TT* y, const std::string& bn, int relu, TT* res, const st
   for (const char* sfx : {".running_mean", ".running_var"}) t->add_bound(bn + sfx, C, 1);
   TT* z = new_tensor(t, zname, C, H);
   YB_PROPAGATE(alloc_data(t, z));
-  float* sums = stats_take(t, 2 * C);
+  float* sums = stats_take(t, 3 * C);                             // sum d | sum d^2 | pivot  (d = y - pivot: k_colstats)
   float* aff = nullptr;                                            // scale | shift | mean | invstd
   YB_PROPAGATE(dev_alloc(t, (void**)&aff, (size_t)4 * C * 4));
   const int ig = t->bidx.at(bn + ".weight"), ib = t->bidx.at(bn + ".bias"), im = t->bidx.at(bn + ".running_mean"), iv = t->bidx.at(bn + ".running_var");
   const double count = (double)B * H * H;
   const long long rows = y->rows;
   void* yd = y->data; void* zd = z->data; void* rd = res ? res->data : nullptr;
-  FWD_PUSH([=](cudaStream_t s) { return launch_colstats(yd, dt, rows, C, (float*)((char*)t->stats + (size_t)sums), s); });
+  FWD_PUSH([=](cudaStream_t s) { return launch_colstats(yd, dt, rows, C, (float*)((char*)t->stats + (size_t)sums), s, H + 2); });
   FWD_PUSH([=](cudaStream_t s) {
     return launch_bn_finalize((float*)((char*)t->stats + (size_t)sums), C, count, t->bound[ig].data, t->bound[ib].data, t->bound[im].data, t->bound[iv].data,
                               t->hp.bn_momentum, t->hp.bn_eps, aff, aff + C, aff + 2 * C, aff + 3 * C, s);

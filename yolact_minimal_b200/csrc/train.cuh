@@ -26,7 +26,8 @@ int launch_unpack_stem_grad(float* g, float* dst, float scale, cudaStream_t s);
 int launch_unpack_wgrad(const UnpackDesc* d_descs, int n, cudaStream_t s);
 
 // ---- batch-statistics BatchNorm ----
-int launch_colstats(const void* x, int dt, long long rows, int C, float* sums /*[2C], pre-zeroed*/, cudaStream_t s);
+int launch_colstats(const void* x, int dt, long long rows, int C, float* sums /*[2C], pre-zeroed*/, cudaStream_t s,
+                    int pivot_Hp = 0 /* > 0: BN statistics of a haloed [B][Hp][Hp][C] tensor, sums [3C] (k_bn_finalize) */);
 int launch_bn_finalize(const float* sums, int C, double count, const float* gamma, const float* beta, float* run_mean, float* run_var,
                        float momentum, float eps, float* scale, float* shift, float* mean, float* invstd, cudaStream_t s);
 int launch_bn_apply(const void* y, void* z, const void* res, const float* scale, const float* shift, int relu, int dt, int B, int C, int H,

@@ -111,11 +111,14 @@ int launch_unpack_wgrad(const UnpackDesc* d_descs, int n, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// per-channel column sums of a [rows][C] 16-bit matrix:  sums[c] += sum_r f(x),  sums[C + c] += sum_r x^2   (BN statistics;
-// bias gradients use the first half only).  Halo rows are zero and contribute nothing.
+// per-channel column sums of a [rows][C] 16-bit matrix:  sums[c] += sum_r x,  sums[C + c] += sum_r x^2   (bias gradients use the
+// first half only).  Halo rows are zero and contribute nothing.
+// BN statistics (kPivot, x haloed [B][Hp][Hp][C]): the sums are taken of d = x - p, p = the channel's first interior value (stored
+// to sums[2C + c]), so that  var = sum d^2 / N - (sum d / N)^2  does not cancel when |mean| >> std (the plain one-pass
+// sum x^2 / N - mean^2 loses (mean / std)^2 of its fp32 precision).  Halo rows are summed unshifted: zero, as before.
 // ------------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(256) k_colstats(const T* __restrict__ x, long long rows, int C, int rows_per_block, float* __restrict__ sums) {
+template <typename T, bool kPivot>
+__global__ void __launch_bounds__(256) k_colstats(const T* __restrict__ x, long long rows, int C, int rows_per_block, float* __restrict__ sums, int Hp) {
   extern __shared__ float sh[];                                   // [2][Cb]
   const int CV = C >> 3;                                          // 8-channel vectors per row
   const int cvb = CV < 256 ? CV : 256;                            // vectors per block
@@ -130,11 +133,30 @@ __global__ void __launch_bounds__(256) k_colstats(const T* __restrict__ x, long 
   const long long r0 = (long long)blockIdx.y * rows_per_block;
   const long long r1 = r0 + rows_per_block < rows ? r0 + rows_per_block : rows;
   if (cv < CV && lane < rl) {
+    float p[8];
+#pragma unroll
+    for (int e = 0; e < 8; ++e) p[e] = 0.f;
+    if (kPivot) {
+      VecIO<T>::load(x + (long long)(Hp + 1) * C + cv * 8, p);
+      if (blockIdx.y == 0 && lane == 0) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e) sums[2 * C + cv * 8 + e] = p[e];
+      }
+    }
+    const unsigned plane = (unsigned)Hp * (unsigned)Hp;
     for (long long r = r0 + lane; r < r1; r += rl) {
       float v[8];
       VecIO<T>::load(x + r * C + cv * 8, v);
+      bool halo = true;
+      if (kPivot) {
+        const unsigned rr = (unsigned)r % plane, yp = rr / (unsigned)Hp, xp = rr - yp * (unsigned)Hp;
+        halo = yp == 0 || xp == 0 || yp == (unsigned)Hp - 1 || xp == (unsigned)Hp - 1;
+      }
 #pragma unroll
-      for (int e = 0; e < 8; ++e) { s1[e] += v[e]; s2[e] = fmaf(v[e], v[e], s2[e]); }
+      for (int e = 0; e < 8; ++e) {
+        const float d = halo ? v[e] : v[e] - p[e];
+        s1[e] += d; s2[e] = fmaf(d, d, s2[e]);
+      }
     }
     const int lc = (threadIdx.x % cvb) * 8;
 #pragma unroll
@@ -147,8 +169,9 @@ __global__ void __launch_bounds__(256) k_colstats(const T* __restrict__ x, long 
   }
 }
 
-int launch_colstats(const void* x, int dt, long long rows, int C, float* sums, cudaStream_t s) {
+int launch_colstats(const void* x, int dt, long long rows, int C, float* sums, cudaStream_t s, int pivot_Hp) {
   YB_REQUIRE(C % 8 == 0, YB_ERR_UNSUPPORTED, "colstats: C=%d", C);
+  YB_REQUIRE(rows < (1LL << 32), YB_ERR_UNSUPPORTED, "colstats: %lld rows", rows);
   const int CV = C / 8, cvb = CV < 256 ? CV : 256;
   const int bx = ceil_div(CV, cvb);
   long long want = (long long)kSmCount * 8 / bx;
@@ -156,19 +179,22 @@ int launch_colstats(const void* x, int dt, long long rows, int C, float* sums, c
   int rpb = (int)((rows + want - 1) / want);
   if (rpb < 64) rpb = 64;
   dim3 grid(bx, (unsigned)((rows + rpb - 1) / rpb));
-  YB_DISPATCH16(dt, (k_colstats<T><<<grid, 256, 2 * cvb * 8 * sizeof(float), s>>>((const T*)x, rows, C, rpb, sums)));
+  if (pivot_Hp > 0) YB_DISPATCH16(dt, (k_colstats<T, true><<<grid, 256, 2 * cvb * 8 * sizeof(float), s>>>((const T*)x, rows, C, rpb, sums, pivot_Hp)));
+  else YB_DISPATCH16(dt, (k_colstats<T, false><<<grid, 256, 2 * cvb * 8 * sizeof(float), s>>>((const T*)x, rows, C, rpb, sums, 0)));
   YB_CHECK_LAUNCH();
   return YB_OK;
 }
 
-// batch statistics -> affine (scale, shift), saved (mean, invstd), running-stat update (torch: momentum 0.1, unbiased variance)
+// batch statistics (pivot-shifted sums of launch_colstats(.., pivot_Hp): [sum d | sum d^2 | pivot]) -> affine (scale, shift),
+// saved (mean, invstd), running-stat update (torch: momentum 0.1, unbiased variance)
 __global__ void k_bn_finalize(const float* __restrict__ sums, int C, double count, const float* __restrict__ gamma, const float* __restrict__ beta,
                               float* __restrict__ run_mean, float* __restrict__ run_var, float momentum, float eps,
                               float* __restrict__ scale, float* __restrict__ shift, float* __restrict__ mean, float* __restrict__ invstd) {
   const int c = blockIdx.x * 256 + threadIdx.x;
   if (c >= C) return;
-  const double m = (double)sums[c] / count;
-  double var = (double)sums[C + c] / count - m * m;
+  const double md = (double)sums[c] / count;
+  const double m = (double)sums[2 * C + c] + md;
+  double var = (double)sums[C + c] / count - md * md;
   if (var < 0) var = 0;
   const float is = (float)(1.0 / sqrt(var + (double)eps));
   mean[c] = (float)m; invstd[c] = is;
