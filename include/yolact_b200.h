@@ -250,6 +250,60 @@ YB_API int yb_net_forward(yb_net* net, const float* img, int batch,
 YB_API int yb_net_read_activation(yb_net* net, const char* name, int batch, float* out, int64_t out_count,
                            int* C, int* H, int* W, void* stream);
 
+/* Debug: the finalized forward op by op (tests).  The program is the list of ops yb_net_forward runs, after the fusion of
+ * bottleneck pairs; ops read and write activations by id.  yb_net_forward(...) == yb_net_forward_range(..., 0, num_ops, ...). */
+typedef enum {
+  YB_OP_STEM = 0, YB_OP_POOL, YB_OP_SPLIT, YB_OP_CONV, YB_OP_UPADD, YB_OP_UP2X, YB_OP_HEADFIN, YB_OP_PATCH_EMBED, YB_OP_LN,
+  YB_OP_ATTN, YB_OP_MERGE_LN, YB_OP_BNECK
+} yb_op_kind;
+
+typedef struct {
+  int kind;                            /* yb_op_kind */
+  int in, out, res, aux, in2, out2;    /* activation ids, -1 = none.  STEM: aux = the space-to-depth image; UPADD: out is updated in
+                                          place; BNECK: out = x', out2 = t1 of the next block, in2 = the folded downsample's input */
+  int stride, relu, heads, shift, level;   /* relu: 0 none, 1 ReLU, 2 exact GELU; level: HEADFIN's pyramid level */
+  int convd;                           /* BNECK: 1 = the block's 1x1 downsample convolution is folded into the first GEMM */
+  int out_mode;                        /* CONV: 0 haloed activation, 1 dense fp32 rows */
+  int ext_proto;                       /* CONV: 1 = writes the proto output of the forward (out = -1) */
+  int k, cin, cout, cout_pad;          /* CONV / BNECK: the (first) convolution */
+  int anchor_offset;                   /* HEADFIN: first anchor of the level */
+  /* state-dict names ("" = none; valid until yb_net_destroy): conv weight / bias / BatchNorm prefix (the head's convolution, which
+     concatenates conf | bbox | coef, has none), BNECK's second convolution and folded downsample, Swin parameter vectors
+     (LN / MERGE_LN: weight, bias; ATTN: qkv bias, relative-position table) */
+  const char* w0; const char* b0; const char* bn0;
+  const char* w1; const char* bn1;
+  const char* wd; const char* bnd;
+  const char* p0; const char* p1;
+} yb_op_info;
+
+typedef struct {
+  int C, H;                /* channels, valid side */
+  int planes;              /* parity planes (stride-2 convolution inputs), else 1 */
+  int dtype;               /* yb_precision code of the stored elements */
+  int dense;               /* 1: dense fp32 rows [B*H*H][C] without halo */
+  int pad_rows;            /* rows allocated behind the max_batch images (the stem's space-to-depth image) */
+  int64_t plane_rows;      /* rows between parity planes: max_batch * (H+2)^2 */
+} yb_act_info;
+
+YB_API int yb_net_num_ops(const yb_net* net);
+YB_API int yb_net_op_info(const yb_net* net, int op, yb_op_info* out);
+YB_API int yb_net_num_acts(const yb_net* net);
+YB_API int yb_net_act_info(const yb_net* net, int act, yb_act_info* out);
+/* Copy activation `act` of the first `batch` images exactly as stored into dst (device), `bytes` = its exact size:
+ *   haloed    [planes][batch][(H+2)^2][C] in the act dtype (planes taken at their plane_rows stride), followed by the pad_rows
+ *             rows behind image batch-1 ([pad_rows][C]) when pad_rows > 0
+ *   dense     [batch*H*H][C] fp32 */
+YB_API int yb_net_read_act_raw(yb_net* net, int act, int batch, void* dst, size_t bytes, void* stream);
+/* The packed GEMM operands of op `op` (device copies into w / b; NULL = sizes only):
+ *   which = 0: CONV: [rows][cols] = [Cout rounded up to 64][k*k*Cin_pad] weights (BN folded, act dtype) and [rows] fp32 biases;
+ *              BNECK: conv3, or [W3 | Wd] and b3 + bd with a folded downsample; STEM: the 16-bit [64][256] GEMM weights
+ *   which = 1: BNECK: the next block's conv1 */
+YB_API int yb_net_read_op_weights(yb_net* net, int op, int which, void* w, size_t w_bytes, float* b, size_t b_bytes, int* rows, int* cols,
+                                  void* stream);
+/* ops [first, last) of yb_net_forward, exactly as it runs them (arguments as there) */
+YB_API int yb_net_forward_range(yb_net* net, const float* img, int batch, int first, int last, float* cls, float* box, float* coef,
+                                float* proto, void* stream);
+
 /* Per-kernel timing of yb_net_forward with CUDA events on the launching stream (bench.py's
  * roofline numbers).  While enabled every forward records one event per layer; yb_net_profile
  * synchronises, aggregates the layers by kernel ("conv_tc", "conv_simt", "stem", ...) over all

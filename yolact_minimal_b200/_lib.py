@@ -50,6 +50,17 @@ class TrainHparams(C.Structure):
                 ('bn_momentum', C.c_float), ('bn_eps', C.c_float)]
 
 
+class OpInfo(C.Structure):
+    _fields_ = [(n, C.c_int) for n in ('kind', 'in_', 'out', 'res', 'aux', 'in2', 'out2', 'stride', 'relu', 'heads', 'shift', 'level',
+                                      'convd', 'out_mode', 'ext_proto', 'k', 'cin', 'cout', 'cout_pad', 'anchor_offset')] + \
+               [(n, C.c_char_p) for n in ('w0', 'b0', 'bn0', 'w1', 'bn1', 'wd', 'bnd', 'p0', 'p1')]
+
+
+class ActInfo(C.Structure):
+    _fields_ = [('C', C.c_int), ('H', C.c_int), ('planes', C.c_int), ('dtype', C.c_int), ('dense', C.c_int), ('pad_rows', C.c_int),
+                ('plane_rows', C.c_int64)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/yolact_b200.h
 PROTOTYPES = {
     'yb_version': (C.c_int, []),
@@ -93,6 +104,13 @@ PROTOTYPES = {
     'yb_net_forward': (C.c_int, [vp, vp, C.c_int, vp, vp, vp, vp, vp]),
     'yb_net_read_activation': (C.c_int, [vp, C.c_char_p, C.c_int, vp, C.c_int64, C.POINTER(C.c_int),
                                          C.POINTER(C.c_int), C.POINTER(C.c_int), vp]),
+    'yb_net_num_ops': (C.c_int, [vp]),
+    'yb_net_op_info': (C.c_int, [vp, C.c_int, C.POINTER(OpInfo)]),
+    'yb_net_num_acts': (C.c_int, [vp]),
+    'yb_net_act_info': (C.c_int, [vp, C.c_int, C.POINTER(ActInfo)]),
+    'yb_net_read_act_raw': (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_size_t, vp]),
+    'yb_net_read_op_weights': (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_size_t, vp, C.c_size_t, C.POINTER(C.c_int), C.POINTER(C.c_int), vp]),
+    'yb_net_forward_range': (C.c_int, [vp, vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]),
     'yb_net_set_profiling': (C.c_int, [vp, C.c_int]),
     'yb_net_profile': (C.c_int, [vp, C.POINTER(ProfEntry), C.c_int, C.POINTER(C.c_int)]),
     'yb_conv2d': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp]),

@@ -739,24 +739,22 @@ extern "C" int yb_net_set_anchors(yb_net* net, const float* anchors_host, int nu
   return YB_OK;
 }
 
-extern "C" int yb_net_forward(yb_net* net, const float* img, int batch, float* cls, float* box, float* coef, float* proto,
-                              void* stream_) {
-  YB_REQUIRE(net && img && cls && box && coef && proto, YB_ERR_INVALID, "yb_net_forward: NULL argument");
-  YB_REQUIRE(net->finalized, YB_ERR_STATE, "yb_net_forward: call yb_net_finalize first");
-  YB_REQUIRE(batch >= 1 && batch <= net->max_batch, YB_ERR_INVALID, "yb_net_forward: batch=%d outside [1,%d]", batch, net->max_batch);
-  cudaStream_t s = (cudaStream_t)stream_;
+namespace {
+
+// ops [first, last) of the program; per-op profiling events only for a whole forward
+int forward_ops(yb_net* net, const float* img, int batch, int first, int last, float* cls, float* box, float* coef, float* proto,
+                cudaStream_t s) {
   const yb_net_config& cfg = net->cfg;
   std::vector<cudaEvent_t>* evs = nullptr;
-  if (net->profiling && net->prof_sets.size() < 512) {
+  if (net->profiling && net->prof_sets.size() < 512 && first == 0 && last == (int)net->ops.size()) {
     net->prof_sets.emplace_back(net->ops.size() + 1);
     net->prof_batch.push_back(batch);
     evs = &net->prof_sets.back();
     for (auto& e : *evs) YB_CHECK_CUDA(cudaEventCreate(&e));
     YB_CHECK_CUDA(cudaEventRecord((*evs)[0], s));
   }
-  int op_index = 0;
-  for (const Op& o : net->ops) {
-    ++op_index;
+  for (int op_index = first + 1; op_index <= last; ++op_index) {
+    const Op& o = net->ops[op_index - 1];
     switch (o.kind) {
       case OP_STEM:
         if (o.tc) {
@@ -829,6 +827,26 @@ extern "C" int yb_net_forward(yb_net* net, const float* img, int batch, float* c
     if (evs) YB_CHECK_CUDA(cudaEventRecord((*evs)[op_index], s));
   }
   return YB_OK;
+}
+
+}  // namespace
+
+extern "C" int yb_net_forward(yb_net* net, const float* img, int batch, float* cls, float* box, float* coef, float* proto,
+                              void* stream_) {
+  YB_REQUIRE(net && img && cls && box && coef && proto, YB_ERR_INVALID, "yb_net_forward: NULL argument");
+  YB_REQUIRE(net->finalized, YB_ERR_STATE, "yb_net_forward: call yb_net_finalize first");
+  YB_REQUIRE(batch >= 1 && batch <= net->max_batch, YB_ERR_INVALID, "yb_net_forward: batch=%d outside [1,%d]", batch, net->max_batch);
+  return forward_ops(net, img, batch, 0, (int)net->ops.size(), cls, box, coef, proto, (cudaStream_t)stream_);
+}
+
+extern "C" int yb_net_forward_range(yb_net* net, const float* img, int batch, int first, int last, float* cls, float* box, float* coef,
+                                    float* proto, void* stream_) {
+  YB_REQUIRE(net && img && cls && box && coef && proto, YB_ERR_INVALID, "yb_net_forward_range: NULL argument");
+  YB_REQUIRE(net->finalized, YB_ERR_STATE, "yb_net_forward_range: call yb_net_finalize first");
+  YB_REQUIRE(batch >= 1 && batch <= net->max_batch, YB_ERR_INVALID, "yb_net_forward_range: batch=%d outside [1,%d]", batch, net->max_batch);
+  YB_REQUIRE(first >= 0 && first <= last && last <= (int)net->ops.size(), YB_ERR_INVALID, "yb_net_forward_range: ops [%d,%d) of %d", first,
+             last, (int)net->ops.size());
+  return forward_ops(net, img, batch, first, last, cls, box, coef, proto, (cudaStream_t)stream_);
 }
 
 extern "C" int yb_net_set_profiling(yb_net* net, int enable) {
@@ -923,6 +941,102 @@ extern "C" int yb_net_read_activation(yb_net* net, const char* name, int batch, 
   if (!out) return YB_OK;
   YB_REQUIRE(out_count >= (int64_t)batch * a.C * a.H * a.H, YB_ERR_INVALID, "yb_net_read_activation: output too small");
   return launch_read_activation(act_ptr(net, it->second), a.dt, batch, a.C, a.H, out, (cudaStream_t)stream);
+}
+
+// ---- debug: the program op by op -----------------------------------------------------------------
+static_assert((int)OP_STEM == YB_OP_STEM && (int)OP_CONV == YB_OP_CONV && (int)OP_HEADFIN == YB_OP_HEADFIN && (int)OP_ATTN == YB_OP_ATTN &&
+              (int)OP_BNECK == YB_OP_BNECK, "yb_op_kind mirrors OpKind");
+
+extern "C" int yb_net_num_ops(const yb_net* net) { return net ? (int)net->ops.size() : 0; }
+extern "C" int yb_net_num_acts(const yb_net* net) { return net ? (int)net->acts.size() : 0; }
+
+extern "C" int yb_net_op_info(const yb_net* net, int i, yb_op_info* out) {
+  YB_REQUIRE(net && out, YB_ERR_INVALID, "yb_net_op_info: NULL argument");
+  YB_REQUIRE(net->finalized, YB_ERR_STATE, "yb_net_op_info: net not finalized");
+  YB_REQUIRE(i >= 0 && i < (int)net->ops.size(), YB_ERR_INVALID, "yb_net_op_info: op %d of %d", i, (int)net->ops.size());
+  const Op& o = net->ops[i];
+  memset(out, 0, sizeof(*out));
+  out->kind = (int)o.kind;
+  out->in = o.in; out->out = o.out; out->res = o.res; out->aux = o.aux; out->in2 = o.in2; out->out2 = o.out2;
+  out->stride = o.stride; out->relu = o.relu; out->heads = o.heads; out->shift = o.shift; out->level = o.level;
+  out->convd = o.convd >= 0 ? 1 : 0;
+  out->out_mode = o.out_mode; out->ext_proto = o.ext == EXT_PROTO ? 1 : 0;
+  out->anchor_offset = o.kind == OP_HEADFIN ? net->level_off[o.level] : 0;
+  static const char* kNone = "";
+  out->w0 = out->b0 = out->bn0 = out->w1 = out->bn1 = out->wd = out->bnd = kNone;
+  out->p0 = o.p0.c_str(); out->p1 = o.p1.c_str();
+  if (o.conv >= 0) {
+    const ConvW& c = net->convs[o.conv];
+    out->k = c.k; out->cin = c.Cin; out->cout = c.Cout; out->cout_pad = c.Cout_pad;
+    out->w0 = c.wname.c_str(); out->b0 = c.bname.c_str(); out->bn0 = c.bnname.c_str();
+  }
+  if (o.conv2 >= 0) { out->w1 = net->convs[o.conv2].wname.c_str(); out->bn1 = net->convs[o.conv2].bnname.c_str(); }
+  if (o.convd >= 0) { out->wd = net->convs[o.convd].wname.c_str(); out->bnd = net->convs[o.convd].bnname.c_str(); }
+  return YB_OK;
+}
+
+extern "C" int yb_net_act_info(const yb_net* net, int act, yb_act_info* out) {
+  YB_REQUIRE(net && out, YB_ERR_INVALID, "yb_net_act_info: NULL argument");
+  YB_REQUIRE(net->finalized, YB_ERR_STATE, "yb_net_act_info: net not finalized");
+  YB_REQUIRE(act >= 0 && act < (int)net->acts.size(), YB_ERR_INVALID, "yb_net_act_info: act %d of %d", act, (int)net->acts.size());
+  const ActBuf& a = net->acts[act];
+  memset(out, 0, sizeof(*out));
+  out->C = a.C; out->H = a.H; out->planes = a.planes; out->dtype = a.dt; out->dense = a.dense_f32 ? 1 : 0; out->pad_rows = a.pad_rows;
+  out->plane_rows = (int64_t)net->max_batch * (a.H + 2) * (a.H + 2);
+  return YB_OK;
+}
+
+extern "C" int yb_net_read_act_raw(yb_net* net, int act, int batch, void* dst, size_t bytes, void* stream) {
+  YB_REQUIRE(net && dst, YB_ERR_INVALID, "yb_net_read_act_raw: NULL argument");
+  YB_REQUIRE(net->finalized, YB_ERR_STATE, "yb_net_read_act_raw: net not finalized");
+  YB_REQUIRE(act >= 0 && act < (int)net->acts.size(), YB_ERR_INVALID, "yb_net_read_act_raw: act %d of %d", act, (int)net->acts.size());
+  YB_REQUIRE(batch >= 1 && batch <= net->max_batch, YB_ERR_INVALID, "yb_net_read_act_raw: batch=%d outside [1,%d]", batch, net->max_batch);
+  const ActBuf& a = net->acts[act];
+  YB_REQUIRE(a.slot >= 0, YB_ERR_STATE, "yb_net_read_act_raw: act %d is never used", act);
+  cudaStream_t s = (cudaStream_t)stream;
+  const char* src = (const char*)act_ptr(net, act);
+  if (a.dense_f32) {
+    const size_t n = (size_t)batch * a.H * a.H * a.C * 4;
+    YB_REQUIRE(bytes == n, YB_ERR_INVALID, "yb_net_read_act_raw: %zu bytes, act %d has %zu", bytes, act, n);
+    YB_CHECK_CUDA(cudaMemcpyAsync(dst, src, n, cudaMemcpyDeviceToDevice, s));
+    return YB_OK;
+  }
+  const size_t row = (size_t)a.C * dtype_size(a.dt), img_rows = (size_t)(a.H + 2) * (a.H + 2);
+  const size_t part = (size_t)batch * img_rows * row, pitch = (size_t)net->max_batch * img_rows * row;
+  const size_t n = part * a.planes + (size_t)a.pad_rows * row;
+  YB_REQUIRE(bytes == n, YB_ERR_INVALID, "yb_net_read_act_raw: %zu bytes, act %d has %zu", bytes, act, n);
+  YB_CHECK_CUDA(cudaMemcpy2DAsync(dst, part, src, pitch, part, a.planes, cudaMemcpyDeviceToDevice, s));
+  if (a.pad_rows) YB_CHECK_CUDA(cudaMemcpyAsync((char*)dst + part * a.planes, src + part, (size_t)a.pad_rows * row, cudaMemcpyDeviceToDevice, s));
+  return YB_OK;
+}
+
+extern "C" int yb_net_read_op_weights(yb_net* net, int op, int which, void* w, size_t w_bytes, float* b, size_t b_bytes, int* rows, int* cols,
+                                      void* stream) {
+  YB_REQUIRE(net && rows && cols, YB_ERR_INVALID, "yb_net_read_op_weights: NULL argument");
+  YB_REQUIRE(net->finalized, YB_ERR_STATE, "yb_net_read_op_weights: net not finalized");
+  YB_REQUIRE(op >= 0 && op < (int)net->ops.size(), YB_ERR_INVALID, "yb_net_read_op_weights: op %d of %d", op, (int)net->ops.size());
+  const Op& o = net->ops[op];
+  const void* dw = nullptr; const float* db = nullptr;
+  if (o.kind == OP_STEM && which == 0) {
+    YB_REQUIRE(o.tc, YB_ERR_UNSUPPORTED, "yb_net_read_op_weights: the stem runs on its fp32 kernel");
+    dw = net->d_stem_w16; db = net->d_stem_b16; *rows = 64; *cols = 256;
+  } else if ((o.kind == OP_CONV || o.kind == OP_BNECK) && which == 0) {
+    const ConvW& c = net->convs[o.conv];
+    if (o.convd >= 0) { dw = o.d_wcat; db = o.d_bcat; *rows = c.Cout; *cols = c.Cin + net->convs[o.convd].Cin; }
+    else { dw = c.d_w; db = c.d_b; *rows = (c.Cout_pad + 63) / 64 * 64; *cols = c.k * c.k * c.Cin_pad; }
+  } else if (o.kind == OP_BNECK && which == 1) {
+    const ConvW& c = net->convs[o.conv2];
+    dw = c.d_w; db = c.d_b; *rows = (c.Cout_pad + 63) / 64 * 64; *cols = c.k * c.k * c.Cin_pad;
+  } else {
+    YB_REQUIRE(false, YB_ERR_INVALID, "yb_net_read_op_weights: op %d (kind %d) has no GEMM %d", op, (int)o.kind, which);
+  }
+  if (!w && !b) return YB_OK;
+  const size_t nw = (size_t)*rows * *cols * dtype_size(net->act_dt), nb = (size_t)*rows * 4;
+  YB_REQUIRE(w && b && w_bytes == nw && b_bytes == nb, YB_ERR_INVALID, "yb_net_read_op_weights: buffers of %zu / %zu bytes, need %zu / %zu",
+             w_bytes, b_bytes, nw, nb);
+  YB_CHECK_CUDA(cudaMemcpyAsync(w, dw, nw, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  YB_CHECK_CUDA(cudaMemcpyAsync(b, db, nb, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return YB_OK;
 }
 
 extern "C" const float* yb_net_last_proto(const yb_net* net) { return net ? net->d_proto : nullptr; }
