@@ -145,10 +145,21 @@ __device__ __forceinline__ void named_barrier_sync(int id, int threads) { asm vo
 __device__ __forceinline__ uint32_t lds32(uint32_t a) { uint32_t v; asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
 __device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
 __device__ __forceinline__ void sts64(uint32_t a, float x, float y) { asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(x), "f"(y) : "memory"); }
+__device__ __forceinline__ float2 lds64(uint32_t a) {
+  float2 v;
+  asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(a) : "memory");
+  return v;
+}
 __device__ __forceinline__ float4 lds128(uint32_t a) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
   return v;
+}
+// non-tensor bulk copy global -> shared (16-byte aligned, a multiple of 16 bytes), its bytes counted on `bar`
+__device__ __forceinline__ void bulk_load(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)), "l"(src),
+               "r"(bytes), "r"(smem_u32(bar))
+               : "memory");
 }
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1)
@@ -511,9 +522,32 @@ struct BnParams {
   const float* b3;
   const float* b1;
   void* t1;
+#ifdef YB_BNECK_TRACE
+  unsigned long long* trace;
+#endif
 };
 
+// Trace build (tools/trace_bneck.cu; the library never defines YB_BNECK_TRACE): thread 0 of each consumer warpgroup writes
+// %globaltimer stamps to trace[((cta * 2 + warpgroup) * BN_TRACE_TILES + tile) * BN_TRACE_SLOTS + slot] for the launch that
+// bn_trace_buf points at.  Slots: 0 tile start; 1 + 5c + {0 A(c) issued, 1 A(c) drained, 2 x_full waited, 3 E(c) done, 4 B(c)
+// issued}; BN_TRACE_T1 the t1 epilogue's start, BN_TRACE_T1 + 1 its end.
+#ifdef YB_BNECK_TRACE
+constexpr int BN_TRACE_TILES = 8, BN_TRACE_SLOTS = 44, BN_TRACE_T1 = 41;
+unsigned long long* bn_trace_buf = nullptr;
+#define BN_TRACE(slot)                                                                                                     \
+  do {                                                                                                                     \
+    if (p.trace && t == 0 && i < BN_TRACE_TILES) {                                                                         \
+      unsigned long long ns_;                                                                                              \
+      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns_));                                                              \
+      p.trace[(((size_t)blockIdx.x * 2 + cw) * BN_TRACE_TILES + i) * BN_TRACE_SLOTS + (slot)] = ns_;                      \
+    }                                                                                                                      \
+  } while (0)
+#else
+#define BN_TRACE(slot) do { } while (0)
+#endif
+
 constexpr uint32_t BN_X_BYTES = 2 * TC_A_STAGE;                  // one x buffer: 128 rows x 128 channels
+constexpr uint32_t BN_B3_BYTES = 128 * 4;                        // b3 of one chunk, beside each x buffer
 constexpr uint32_t BN_SLOT = TC_A_STAGE;                         // one ring slot: 128 rows x 128 B
 
 template <bool F16, int COUT>
@@ -527,7 +561,8 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint8_t* sT2 = smem;                                         // [kbA][128 rows x 128 B]
   uint8_t* sX = sT2 + (size_t)p.kbA * TC_A_STAGE;              // [2 buffers][2 k-blocks][128 rows x 128 B]
-  uint8_t* sRing = sX + 2 * BN_X_BYTES;                        // [slots][BN_SLOT]
+  uint8_t* sB3 = sX + 2 * BN_X_BYTES;                          // [2 buffers][128 floats]: b3 of the chunk in x buffer b
+  uint8_t* sRing = sB3 + 2 * BN_B3_BYTES;                      // [slots][BN_SLOT]
   uint64_t* full = reinterpret_cast<uint64_t*>(sRing + (size_t)p.slots * BN_SLOT);
   uint64_t* empty = full + TC_MAX_STAGES;
   uint64_t* t2_full = empty + TC_MAX_STAGES;
@@ -561,13 +596,12 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
         for (int c = 0; c < p.nch; ++c, ++q) {
           const int xb = q & 1;
           mbar_wait(&x_empty[xb], (uint32_t)((q >> 1) & 1) ^ 1u);   // B(q-2) has retired and xo's store has read the buffer
-          if (p.has_res) {
-            mbar_expect_tx(&x_full[xb], BN_X_BYTES);
+          // the chunk's b3 with it (folded branch: no residual, the buffer only holds x')
+          mbar_expect_tx(&x_full[xb], (p.has_res ? BN_X_BYTES : 0u) + BN_B3_BYTES);
+          bulk_load(sB3 + (size_t)xb * BN_B3_BYTES, p.b3 + c * 128, BN_B3_BYTES, &x_full[xb]);
+          if (p.has_res)
             for (int kb = 0; kb < 2; ++kb)
               tma_load_2d(sX + (size_t)xb * BN_X_BYTES + (size_t)kb * TC_A_STAGE, &tmX, c * 128 + kb * TC_BK, row0, &x_full[xb]);
-          } else {
-            mbar_arrive(&x_full[xb]);                               // folded branch: no residual, the buffer only holds x'
-          }
           for (int kb = 0; kb < p.kbA; ++kb) {                      // W3 rows c*128 .., k-block kb
             mbar_wait(&empty[stage], phase ^ 1);
             mbar_expect_tx(&full[stage], TC_A_STAGE);
@@ -602,6 +636,7 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
     };
     int q = 0;
     for (int i = 0, tile = (int)blockIdx.x; tile < p.m_tiles; ++i, tile += (int)gridDim.x) {
+      BN_TRACE(0);
       long long m[2];
       bool valid[2], zero[2];
 #pragma unroll
@@ -636,18 +671,23 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
           if (xpend >= 0) { release_x(xpend); xpend = -1; }
           if (++stage == p.slots) { stage = 0; phase ^= 1; }
         }
+        BN_TRACE(1 + 5 * c);
         wgmma_wait<0>();
         acc_fence<64>(accA);
+        BN_TRACE(2 + 5 * c);
         release(prev);
         prev = -1;
         if (c == p.nch - 1 && signal) mbar_arrive(t2_empty);
         // ---- E(c): rows r, r + 8 of this thread, columns c*128 + 8j + 2 (lane % 4) + {0, 1} ----
-        mbar_wait(&x_full[xb], (uint32_t)((q >> 1) & 1));          // x_c has landed (and the buffer is free)
+        mbar_wait(&x_full[xb], (uint32_t)((q >> 1) & 1));          // x_c and its b3 have landed (and the buffer is free)
+        BN_TRACE(3 + 5 * c);
         const uint32_t sXw = smem_u32(sX + (size_t)xb * BN_X_BYTES + (size_t)cw * (TC_A_STAGE / 2));   // this warpgroup's 64 rows
-        const float2* b3 = reinterpret_cast<const float2*>(p.b3 + c * 128) + (lane & 3);
+        // b3 from shared memory: per column group a global load would miss the small L1 left beside the shared-memory carve-out and
+        // wait out an L2 latency behind the previous group's shared-memory store
+        const uint32_t b3 = smem_u32(sB3 + (size_t)xb * BN_B3_BYTES) + 8u * (lane & 3);
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-          const float2 b = __ldg(b3 + 4 * j);                      // columns c*128 + 8j + 2 (lane % 4) + {0, 1}: shared by both rows
+          const float2 b = lds64(b3 + 32u * j);                    // columns c*128 + 8j + 2 (lane % 4) + {0, 1}: shared by both rows
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const int r = warp * 16 + (lane >> 2) + 8 * h;        // row in this warpgroup's 64-row slab
@@ -664,6 +704,7 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
         }
         fence_async_smem();
         named_barrier_sync(1 + cw, 128);                           // the whole x' chunk of this warpgroup is staged
+        BN_TRACE(4 + 5 * c);
         if (t == 0) {
           const int row = tile * TC_BM + cw * 64;
 #pragma unroll
@@ -689,10 +730,12 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
           prev = stage;
           if (++stage == p.slots) { stage = 0; phase ^= 1; }
         }
+        BN_TRACE(5 + 5 * c);
         xpend = xb;
       }
       wgmma_wait<0>();
       acc_fence<COUT / 2>(accB);
+      BN_TRACE(BN_TRACE_T1);
       release(prev);
       prev = -1;
       release_x(xpend);
@@ -715,6 +758,7 @@ k_bneck_tc(const __grid_constant__ CUtensorMap tmT2, const __grid_constant__ CUt
             reinterpret_cast<uint2*>((uint16_t*)p.t1 + m[h] * COUT)[4 * g + 2 * (lane & 1) + ((lane >> 1) & 1)] = zero[h] ? make_uint2(0u, 0u) : make_uint2(v0, v1);
         }
       }
+      BN_TRACE(BN_TRACE_T1 + 1);
     }
     if (t == 0) bulk_wait0();                                      // xo's stores are complete before the CTA exits
   }
@@ -991,7 +1035,7 @@ int bneck_plan_create(const BneckArgs& a, int max_batch, BnPlan** out) {
   BnPlan* pl = new BnPlan();
   pl->Cin = a.Cin; pl->Cout = a.Cout; pl->Cd = a.Cd;
   const int kbA = (a.Cin + a.Cd) / 64;
-  const size_t fixed = 1024 /*align*/ + (2 * TC_MAX_STAGES + 6) * 8 /*barriers*/ + (size_t)kbA * TC_A_STAGE + 2 * BN_X_BYTES;
+  const size_t fixed = 1024 /*align*/ + (2 * TC_MAX_STAGES + 6) * 8 /*barriers*/ + (size_t)kbA * TC_A_STAGE + 2 * (BN_X_BYTES + BN_B3_BYTES);
   int slots = (int)((TC_SMEM_MAX - fixed) / BN_SLOT);
   pl->slots = slots > TC_MAX_STAGES ? TC_MAX_STAGES : slots;
   pl->smem_bytes = fixed + (size_t)pl->slots * BN_SLOT;
@@ -1025,7 +1069,11 @@ int launch_bneck_tc(const BnPlan* pl, const BneckArgs& a, cudaStream_t s) {
   p.Cexp = a.Cexp; p.nch = a.Cexp / 128; p.kbT = pl->Cin / 64; p.kbA = (pl->Cin + pl->Cd) / 64; p.has_res = pl->Cd ? 0 : 1;
   p.slots = pl->slots;
   p.g = a.g; p.b3 = a.b3; p.b1 = a.b1; p.t1 = a.t1;
+#ifdef YB_BNECK_TRACE
+  p.trace = bn_trace_buf;
+#endif
   // xo is written by TMA stores of [64 rows x 64 channels]; the map ends at this launch's last row, so rows >= M stay untouched
+  YB_REQUIRE(((uintptr_t)a.b3 & 15) == 0, YB_ERR_INVALID, "launch_bneck_tc: b3 is not 16-byte aligned (bulk copy)");
   CUtensorMap tmXo;
   YB_PROPAGATE(make_map(&tmXo, a.xo, (uint64_t)a.Cexp, (uint64_t)p.M, 64, a.act_dt == DT_F16));
   static const bool pdl = getenv("YOLACT_B200_NO_PDL") == nullptr;
