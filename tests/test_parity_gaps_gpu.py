@@ -3,7 +3,7 @@
   * the BENCHMARKED configuration (res101_coco 550x550, B=64, fp16 operands) is parity-checked itself:
     images 0 / 31 / 63 of the B=64 output vs the fp32 oracle (<= 1e-2, north_star's 16-bit bound) and
     bit-wise vs B=1 runs of the same images (persistent tile scheduling, CTA-pair tails and arena reuse
-    only show their bugs at large B);
+    only show their bugs at large B); the detections of all 64 images vs the oracle's, bit for bit;
   * N-rank sharded inference: the NCCL-gathered detection records equal the single-GPU detections of the
     concatenated batch bit-for-bit (SURVEY.md 8(e)); needs >= 2 GPUs, skipped otherwise;
   * Fast-NMS decisions within a few ulps of IoU == threshold (SURVEY.md App. B; the kernel decides with a
@@ -54,15 +54,16 @@ def test_bench_config_b64_res101_550_fp16(cuda):
             assert torch.equal(f[b:b + 1], o), f'image {b} {name}: B=64 output differs bit-wise from the B=1 run'
             err = float(np.abs(f[b:b + 1].cpu().numpy() - r).max())
             assert err < 1e-2, f'image {b} {name}: max abs err {err} vs the fp32 oracle'
-    # the timed step's second half: detections of the B=64 batch == detections of the B=1 runs, and index-exact vs the oracle
+    # the timed step's second half: the detections of every image of the B=64 batch equal the oracle's bit for bit
+    # (count, class, anchor, score, box bits, coefficient rows)
     from yolact_minimal_b200.utils.output_utils import detect_batched
+    from test_postprocess_gpu import _check_image
     det = detect_batched(full[0], full[1], full[2], net.anchors, net.cfg)
+    det = {k: v.cpu().numpy() for k, v in det.items() if not k.startswith('_')}
     anchors = net.engine(B).anchors()
-    for b in (0, 31, 63):
-        o = pp.nms(full[0][b].cpu().numpy(), full[1][b].cpu().numpy(), anchors)
-        d = int(det['count'][b])
-        assert o is not None and d == len(o[0])
-        assert np.array_equal(det['cls'][b, :d].cpu().numpy(), o[0]) and np.array_equal(det['anchor'][b, :d].cpu().numpy(), o[3])
+    cls, box, coef = (full[i].float().cpu().numpy() for i in range(3))
+    for b in range(B):
+        _check_image(det, b, pp.nms(cls[b], box[b], anchors), coef[b])
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason='needs >= 2 GPUs')

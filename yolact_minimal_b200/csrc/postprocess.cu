@@ -664,8 +664,13 @@ k_class_fast_nms(const float* __restrict__ cls, int A, int C1, int top_k, float 
 
 // --------------------------------------------------------------------------------------------
 // phase 2 (traditional): greedy per-class NMS in pixel coords   output_utils.py:84-113 +
-// cython_nms.pyx:24-74.  Survivors are found in descending score order, so the loop stops after
-// max_keep of them (only those can reach the cross-class top max_det).
+// cython_nms.pyx:24-74.  Survivors are found in descending score order (ties: larger anchor
+// first), but the cross-class ranking (output_utils.py:115-117, k_final_topk) breaks ties by
+// ascending anchor.  So the class keeps the max_keep best survivors by (score desc, anchor asc):
+// the first max_keep in greedy order, except that the group tied at the max_keep-th score must
+// hold the SMALLEST tied anchors.  After max_keep survivors the loop runs on while the winner ties
+// with that score; each such winner has a smaller anchor than every stored one of the group and
+// replaces the group's oldest (= largest-anchor) entry, so at most max_keep entries are stored.
 // --------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kThreads)
 k_class_hard_nms(int A, int C1, float score_thr, float iou_thr, float img_size, int max_keep, DetectWs ws) {
@@ -680,8 +685,10 @@ k_class_hard_nms(int A, int C1, float score_thr, float iou_thr, float img_size, 
   const float4* cbox = ws.cand_box + (size_t)b * A;
   for (int i = tid; i < n; i += kThreads) { float s = row[i]; s_sc[i] = (s > score_thr) ? s : -INFINITY; }
   __syncthreads();
-  int kept = 0;
-  while (kept < max_keep) {
+  int kept = 0;                                    // stored survivors (<= max_keep)
+  float run_score = -INFINITY;                     // thread 0: score of the last stored survivor,
+  int run_start = 0, replaced = 0;                 //   first slot holding it, tied winners past max_keep
+  while (true) {
     // argmax (score desc, ties: larger anchor first == reversed stable ascending argsort)
     float best = -INFINITY; int besti = -1; int besta = -1;
     for (int i = tid; i < n; i += kThreads) {
@@ -705,16 +712,25 @@ k_class_hard_nms(int A, int C1, float score_thr, float iou_thr, float img_size, 
         int aa = canchor[ii];
         if (s_best[i] > bb || (s_best[i] == bb && aa > ba)) { bb = s_best[i]; bi = ii; ba = aa; }
       }
-      s_win = (bb > -INFINITY) ? bi : -1;
-      if (s_win >= 0) {
-        const size_t o = ((size_t)b * C1 + c) * ws.KC + kept;
+      int win = (bb > -INFINITY) ? bi : -1, slot = kept;
+      if (win >= 0 && kept < max_keep) {
+        if (bb != run_score) { run_score = bb; run_start = kept; }
+      } else if (win >= 0 && bb == run_score) {     // tied with the max_keep-th survivor: replace the group's largest anchor
+        slot = run_start + replaced % (max_keep - run_start);
+        ++replaced;
+      } else {
+        win = -1;                                  // below the cut (or none left): no later survivor can rank in
+      }
+      s_win = win;
+      if (win >= 0) {
+        const size_t o = ((size_t)b * C1 + c) * ws.KC + slot;
         ws.cls_score[o] = bb; ws.cls_anchor[o] = ba; ws.cls_slot[o] = bi;
       }
     }
     __syncthreads();
     const int win = s_win;
     if (win < 0) break;
-    ++kept;
+    if (kept < max_keep) ++kept;
     float4 bw = cbox[win];
     bw = make_float4(__fmul_rn(bw.x, img_size), __fmul_rn(bw.y, img_size), __fmul_rn(bw.z, img_size), __fmul_rn(bw.w, img_size));
     const float aw = area_plus1(bw);
@@ -933,6 +949,10 @@ extern "C" int yb_detect(const float* cls, const float* box, const float* coef, 
   DetectWs ws;
   const size_t need = carve(&ws, (char*)workspace, B, A, C1, KC, p->traditional != 0);
   YB_REQUIRE(workspace_bytes >= need, YB_ERR_INVALID, "yb_detect: workspace %zu < %zu bytes", workspace_bytes, need);
+  if (p->traditional) {                                       // refused before anything is launched or written
+    YB_REQUIRE(A <= 49152, YB_ERR_UNSUPPORTED, "yb_detect(traditional): num_anchors=%d > 49152", A);   // k_class_hard_nms: A scores in shared memory
+    YB_REQUIRE(p->img_size > 0.f, YB_ERR_INVALID, "yb_detect(traditional): img_size must be > 0");
+  }
   cudaStream_t stream = (cudaStream_t)stream_;
 
   YB_CHECK_CUDA(cudaMemsetAsync(ws.cand_count, 0, sizeof(int) * B, stream));
@@ -963,8 +983,6 @@ extern "C" int yb_detect(const float* cls, const float* box, const float* coef, 
     k_class_fast_nms<<<dim3(C1, B), kThreads, 0, stream>>>(cls, A, C1, p->top_k, p->iou_thr, ws);
     YB_CHECK_LAUNCH();
   } else {
-    YB_REQUIRE(A <= 49152, YB_ERR_UNSUPPORTED, "yb_detect(traditional): num_anchors=%d > 49152", A);
-    YB_REQUIRE(p->img_size > 0.f, YB_ERR_INVALID, "yb_detect(traditional): img_size must be > 0");
     const size_t smem = (size_t)A * sizeof(float);
     YB_CHECK_CUDA(cudaFuncSetAttribute(k_class_hard_nms, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_class_hard_nms<<<dim3(C1, B), kThreads, smem, stream>>>(A, C1, p->score_thr, p->iou_thr, p->img_size, p->max_det, ws);
