@@ -182,6 +182,52 @@ YB_API int yb_eval_ap(const yb_eval_params* p, const float* rec_score, const int
 YB_API int yb_val_aug(const uint8_t* img_bgr, int h, int w, int img_size, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Training augmentation -- the pixel work of utils/augmentations.py:230-252 train_aug for a batch, given the
+ * plans drawn on the host by yolact_minimal_b200.utils.augmentations.train_aug_plan (every random draw of
+ * train_aug depends only on shapes and boxes, so the host keeps them and the device only moves pixels).
+ * Per output pixel, a composite gather:
+ *   to_train_size pad/crop -> INTER_LINEAR resize square -> resize (OpenCV coordinates: x taps clamped with
+ *   weight 0 outside, y rows clipped with the weights kept) -> pad to square (image fill norm_mean, mask 0)
+ *   -> crop -> mirror -> photometric transform of the source pixel:
+ *   brightness (+delta, clip 0..255), contrast (*alpha, clip), cv2 float BGR->HSV, S *= saturation (no clip),
+ *   H += hue (wrapped once at > 360 / < 0), cv2 float HSV->BGR, clip 0..255; then (x-mean)/std, BGR->RGB.
+ * Masks use float32 arithmetic, or (mask_u8 = 1, when the cropped image is already square and no pad made the
+ * masks float) OpenCV's 11-bit fixed-point linear weights with its vectorised rounding
+ * ((((h0>>4)*b0>>16) + ((h1>>4)*b1>>16) + 2) >> 2), which leaves them 0/1.
+ *
+ * src: one device buffer holding every image (uint8 BGR HWC [h,w,3]) and its masks (uint8 [num_masks,h,w]).
+ * items / keep are HOST tables (copied into the workspace): item i writes out_img[i] ([B,3,S,S] float32 RGB) and
+ * out_masks rows out_mask .. out_mask+num_keep-1 ([G,S,S] float32, G = sum of num_keep); row k is the source mask
+ * keep[keep_begin + k].  Items are dense: out_mask and keep_begin both equal the sum of num_keep before the item.
+ * Every offset, size and index is checked on the host before anything is launched (YB_ERR_INVALID).  The tables are
+ * then copied through library-owned page-locked staging, so the call queues on the stream without waiting for earlier work;
+ * the caller's tables may be freed when it returns.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct {
+  int64_t img_off;           /* byte offset of the image in src */
+  int64_t mask_off;          /* byte offset of the masks in src */
+  int32_t h, w, num_masks;
+  int32_t brightness_on;     /* 0/1 */
+  float brightness_delta;    /* float32, added when brightness_on */
+  int32_t contrast_on;       /* 0/1 */
+  float contrast_alpha;      /* float32, multiplied when contrast_on */
+  float saturation_scale;
+  float hue_delta;
+  int32_t mirror;            /* 0/1: x -> w-1-x before the crop */
+  int32_t crop_x, crop_y, crop_w, crop_h; /* crop rectangle in the (mirrored) image; (0,0,w,h) when not cropped */
+  int32_t square;            /* max(crop_w, crop_h) */
+  int32_t pad_x, pad_y;      /* offset of the crop in the square */
+  int32_t resize;            /* side after the multi-scale resize */
+  int32_t train_x, train_y;  /* to_train_size: pad offset when resize < img_size, crop offset when resize > img_size, else 0 */
+  int32_t mask_u8;           /* 0 float32 mask arithmetic, 1 OpenCV uint8 fixed point */
+  int32_t out_mask, keep_begin, num_keep;
+} yb_train_aug_item;
+
+YB_API size_t yb_train_aug_workspace_bytes(int n_items, int64_t n_keep);
+YB_API int yb_train_aug(const uint8_t* src, int64_t src_bytes, const yb_train_aug_item* items, int n_items, const int32_t* keep,
+                        int img_size, void* workspace, size_t workspace_bytes, float* out_img, float* out_masks, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Drawing -- the pixel work of utils/output_utils.py:308-369 (draw_img); the box, label and fps drawing stays on the host.
  *   semantic = (sum_i m_i * (ids_i + 1)) mod num_colors     floor modulo (numpy %); num_colors = cfg.num_classes - 1
  *   yb_draw_masks   out = rint(0.4f * palette[semantic] + 0.6f * img) per channel -- cv2.addWeighted(COLORS[semantic], 0.4,

@@ -61,6 +61,15 @@ class ActInfo(C.Structure):
                 ('plane_rows', C.c_int64)]
 
 
+class TrainAugItem(C.Structure):
+    """yb_train_aug_item: one image's augmentation plan as the kernel reads it."""
+    _fields_ = [('img_off', C.c_int64), ('mask_off', C.c_int64)] + \
+               [(n, C.c_int32) for n in ('h', 'w', 'num_masks', 'brightness_on')] + [('brightness_delta', C.c_float)] + \
+               [('contrast_on', C.c_int32), ('contrast_alpha', C.c_float), ('saturation_scale', C.c_float), ('hue_delta', C.c_float)] + \
+               [(n, C.c_int32) for n in ('mirror', 'crop_x', 'crop_y', 'crop_w', 'crop_h', 'square', 'pad_x', 'pad_y', 'resize',
+                                         'train_x', 'train_y', 'mask_u8', 'out_mask', 'keep_begin', 'num_keep')]
+
+
 # name -> (restype, argtypes); every symbol declared in include/yolact_b200.h
 PROTOTYPES = {
     'yb_version': (C.c_int, []),
@@ -78,6 +87,8 @@ PROTOTYPES = {
     'yb_mask_assemble': (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                    vp, C.c_size_t, vp, vp, vp]),
     'yb_val_aug': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp]),
+    'yb_train_aug_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int64]),
+    'yb_train_aug': (C.c_int, [vp, C.c_int64, C.POINTER(TrainAugItem), C.c_int, vp, C.c_int, vp, C.c_size_t, vp, vp, vp]),
     'yb_pack_mask_bits': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
     'yb_mask_iou_bits': (C.c_int, [vp, C.c_int, vp, C.c_int, C.c_int64, vp, vp]),
     'yb_box_iou': (C.c_int, [vp, C.c_int, vp, C.c_int, vp, vp]),

@@ -1,7 +1,21 @@
-"""`val_aug` kept from the reference's utils/augmentations.py:219-227, computed on the GPU by
+"""Augmentation on the GPU.
+
+`val_aug` kept from the reference's utils/augmentations.py:219-227, computed on the GPU by
 yb_val_aug (one fused kernel: pad-to-square with the BGR mean, bilinear resize, normalise,
 BGR->RGB, HWC->CHW).  Takes the uint8 BGR image (numpy HWC, as cv2.imread returns it, or a CUDA
-uint8 tensor) and returns a CUDA float32 tensor [3, val_size, val_size]."""
+uint8 tensor) and returns a CUDA float32 tensor [3, val_size, val_size].
+
+`train_aug` (:230-252) is split in two.  Every random draw it makes depends only on shapes, boxes
+and labels, never on pixel values, so `train_aug_plan` replays those draws on the host (the same
+`random` calls in the same order, the same float64 box arithmetic) and returns a small plan without
+touching a pixel; `train_aug_batch` then applies a batch of plans to the raw uint8 images and masks
+in one yb_train_aug launch.  With the same `random` state the plan's boxes and labels are the
+reference's bit for bit.
+"""
+import ctypes as C
+import random
+from dataclasses import dataclass
+
 import numpy as np
 import torch
 
@@ -22,3 +36,230 @@ def val_aug(img, val_size, device='cuda'):
         _lib.check(_lib.lib().yb_val_aug(img.data_ptr(), h, w, int(val_size), out.data_ptr(),
                                          torch.cuda.current_stream().cuda_stream), 'yb_val_aug')
     return out
+
+
+# ----------------------------------------------------------------------------- train_aug: host planner
+@dataclass
+class TrainAugPlan:
+    """What train_aug does to one image, minus the pixels.  Coordinates follow the reference's stages:
+    `crop` = (x, y, w, h) in the mirrored image, `pad` = (x, y) offset of the crop in the `square`,
+    `train_off` = (x, y) pad offset (resize < train_size) or crop offset (resize > train_size)."""
+    h: int
+    w: int
+    brightness: object          # float delta, or None when the draw skipped it
+    contrast: object            # float alpha, or None
+    saturation: float
+    hue: float
+    mirror: bool
+    crop: tuple
+    square: int
+    pad: tuple
+    resize: int
+    train_size: int
+    train_off: tuple
+    mask_u8: bool               # the masks stay uint8 through the resize (no pad to square happened)
+    keep: np.ndarray            # int64 indices of the source masks that survive, in output order
+    boxes: np.ndarray           # float64 [n,4] in [0,1]
+    labels: np.ndarray          # float64 [n]
+
+
+def _crop_window(ori_h, crop_h, ori_w, crop_w, boxes, keep_ratio=0.3):
+    """utils/augmentations.py:80-124 `crop` without pixels: up to 1000 tries of (x, then y); a box is kept when
+    its intersection with the window covers more than keep_ratio of its area.  The window corners are float32 in
+    the reference and the boxes float64, so the test runs in float64 (a zero-area box gives NaN and never passes).
+    Returns (x1, y1, keep mask, kept intersection boxes relative to the window) or None."""
+    area = (boxes[:, 2] - boxes[:, 0]) * (boxes[:, 3] - boxes[:, 1])
+    for _ in range(1000):
+        x1 = random.randint(0, ori_w - crop_w)
+        y1 = random.randint(0, ori_h - crop_h)
+        lo_x = np.maximum(np.float64(np.float32(x1)), boxes[:, 0])
+        lo_y = np.maximum(np.float64(np.float32(y1)), boxes[:, 1])
+        hi_x = np.minimum(np.float64(np.float32(x1 + crop_w)), boxes[:, 2])
+        hi_y = np.minimum(np.float64(np.float32(y1 + crop_h)), boxes[:, 3])
+        inter = np.clip(hi_x - lo_x, 0, 10000) * np.clip(hi_y - lo_y, 0, 10000)
+        with np.errstate(divide='ignore', invalid='ignore'):
+            keep = inter / area > keep_ratio
+        if keep.any():
+            kept = np.stack([lo_x, lo_y, hi_x, hi_y], axis=1)[keep]
+            kept[:, [0, 2]] -= x1
+            kept[:, [1, 3]] -= y1
+            return x1, y1, keep, kept
+    return None
+
+
+def train_aug_plan(h, w, boxes, labels, train_size):
+    """Draw one image's train_aug plan (utils/augmentations.py:230-252) from Python's `random`, in the reference's
+    order.  boxes: [n,4] x1y1x2y2 pixels (float64), labels: [n].  Returns a TrainAugPlan, or None where the
+    reference returns (None,)*4 (the crop found no window in 1000 tries, or no box survived)."""
+    h, w, S = int(h), int(w), int(train_size)
+    boxes = np.array(boxes, dtype=np.float64).reshape(-1, 4)
+    labels = np.asarray(labels).astype(np.float64).reshape(-1)
+    idx = np.arange(boxes.shape[0])
+    # photometric_distort (:62-77): brightness and contrast each behind a coin, then saturation and hue
+    brightness = random.uniform(-32, 32) if random.randint(0, 1) else None
+    contrast = random.uniform(0.7, 1.3) if random.randint(0, 1) else None
+    saturation = random.uniform(0.7, 1.3)
+    hue = random.uniform(-15., 15.)
+    # random_mirror (:10-17)
+    mirror = bool(random.randint(0, 1))
+    if mirror:
+        boxes[:, [0, 2]] = w - boxes[:, [2, 0]]
+    # random_crop (:127-135): a coin of 1 leaves the image whole
+    crop = (0, 0, w, h)
+    if not random.randint(0, 1):
+        crop_h = int(random.uniform(0.6, 1) * h)
+        crop_w = int(random.uniform(0.6, 1) * w)
+        r = _crop_window(h, crop_h, w, crop_w, boxes)
+        if r is None:
+            return None
+        x1, y1, keep, boxes = r
+        idx, labels = idx[keep], labels[keep]
+        crop = (x1, y1, crop_w, crop_h)
+    # pad_to_square (:138-165): a random offset along the short side; a square crop is left alone (masks stay uint8)
+    cw, ch = crop[2], crop[3]
+    square, pad = max(cw, ch), (0, 0)
+    if ch < cw:
+        pad = (0, random.randint(0, cw - ch))
+        boxes[:, [1, 3]] += pad[1]
+    elif ch > cw:
+        pad = (random.randint(0, ch - cw), 0)
+        boxes[:, [0, 2]] += pad[0]
+    # multi_scale_resize (:168-189)
+    resize = random.randint(8, 24) * 32
+    boxes *= resize / square
+    # to_train_size (:192-209): pad (y, then x) or crop (the crop loop again, x then y)
+    train_off = (0, 0)
+    if resize < S:
+        ty = random.randint(0, S - resize)
+        tx = random.randint(0, S - resize)
+        boxes[:, [1, 3]] += ty
+        boxes[:, [0, 2]] += tx
+        train_off = (tx, ty)
+    elif resize > S:
+        r = _crop_window(resize, S, resize, S, boxes)
+        if r is None:
+            return None
+        tx, ty, keep, boxes = r
+        idx, labels = idx[keep], labels[keep]
+        train_off = (tx, ty)
+    # clip_box, remove_small_box (area > 20), to_01_box (:20-35)
+    boxes[:, [0, 2]] = np.clip(boxes[:, [0, 2]], 0, S - 1)
+    boxes[:, [1, 3]] = np.clip(boxes[:, [1, 3]], 0, S - 1)
+    big = (boxes[:, 2] - boxes[:, 0]) * (boxes[:, 3] - boxes[:, 1]) > 20
+    boxes, labels, idx = boxes[big], labels[big], idx[big]
+    if boxes.shape[0] == 0:
+        return None
+    boxes[:, [0, 2]] /= S
+    boxes[:, [1, 3]] /= S
+    return TrainAugPlan(h=h, w=w, brightness=brightness, contrast=contrast, saturation=saturation, hue=hue, mirror=mirror,
+                        crop=tuple(int(v) for v in crop), square=square, pad=pad, resize=resize, train_size=S, train_off=train_off,
+                        mask_u8=(cw == ch), keep=idx.astype(np.int64), boxes=boxes, labels=labels)
+
+
+# ----------------------------------------------------------------------------- train_aug: batch packing + GPU executor
+class PackedTrainBatch:
+    """A batch ready for yb_train_aug: one contiguous uint8 buffer (each image [h,w,3] BGR then its masks [n,h,w]),
+    the item table, the `keep` table and the targets ([n_i,5] float32: boxes in [0,1] then the label).
+
+    It is built in DataLoader workers and sent to the main process, so it holds only picklable types: the buffer is a
+    torch uint8 tensor (it travels through shared memory), the item table a numpy array with yb_train_aug_item's
+    layout, `keep` an int32 numpy array.  With DataLoader(pin_memory=True) the loader's pin thread calls pin_memory()
+    and train_aug_batch copies the buffer to the device asynchronously."""
+
+    ITEM_DTYPE = np.dtype(_lib.TrainAugItem)
+
+    def __init__(self, samples):
+        """samples: list of (img_u8 [h,w,3], masks_u8 [n,h,w], TrainAugPlan)."""
+        sizes = [s[0].nbytes + s[1].nbytes for s in samples]
+        buf = np.empty(sum(sizes), dtype=np.uint8)
+        self.items = np.zeros(len(samples), dtype=self.ITEM_DTYPE)
+        keeps, self.targets, self.num_keep = [], [], []
+        off = rows = 0
+        for i, ((img, masks, plan), size) in enumerate(zip(samples, sizes)):
+            h, w = img.shape[:2]
+            if img.dtype != np.uint8 or img.shape != (plan.h, plan.w, 3) or masks.dtype != np.uint8 or masks.shape[1:] != (h, w):
+                raise ValueError(f'sample {i}: expected uint8 image [{plan.h},{plan.w},3] and uint8 masks [n,{plan.h},{plan.w}], '
+                                 f'got {img.dtype} {img.shape} and {masks.dtype} {masks.shape}')
+            buf[off:off + img.nbytes] = img.reshape(-1)
+            buf[off + img.nbytes:off + size] = masks.reshape(-1)
+            fields = dict(img_off=off, mask_off=off + img.nbytes, h=h, w=w, num_masks=masks.shape[0],
+                          brightness_on=plan.brightness is not None, brightness_delta=np.float32(plan.brightness or 0.0),
+                          contrast_on=plan.contrast is not None, contrast_alpha=np.float32(plan.contrast or 1.0),
+                          saturation_scale=np.float32(plan.saturation), hue_delta=np.float32(plan.hue), mirror=plan.mirror,
+                          crop_x=plan.crop[0], crop_y=plan.crop[1], crop_w=plan.crop[2], crop_h=plan.crop[3], square=plan.square,
+                          pad_x=plan.pad[0], pad_y=plan.pad[1], resize=plan.resize, train_x=plan.train_off[0],
+                          train_y=plan.train_off[1], mask_u8=plan.mask_u8, out_mask=rows, keep_begin=rows, num_keep=len(plan.keep))
+            for k, v in fields.items():
+                self.items[k][i] = v
+            keeps.append(plan.keep)
+            self.targets.append(torch.from_numpy(np.hstack((plan.boxes, plan.labels[:, None])).astype(np.float32)))
+            self.num_keep.append(len(plan.keep))
+            off += size
+            rows += len(plan.keep)
+        self.buffer = torch.from_numpy(buf)
+        self.keep = np.ascontiguousarray(np.concatenate(keeps).astype(np.int32))
+        self.train_size = samples[0][2].train_size
+        if any(s[2].train_size != self.train_size for s in samples):
+            raise ValueError('every plan of a batch must have the same train_size')
+
+    def __len__(self):
+        return len(self.items)
+
+    def pin_memory(self):
+        """Called by DataLoader(pin_memory=True) in its pin thread: page-locks the buffer and the targets."""
+        self.buffer = self.buffer.pin_memory()
+        self.targets = [t.pin_memory() for t in self.targets]
+        return self
+
+    def items_ptr(self):
+        return self.items.ctypes.data_as(C.POINTER(_lib.TrainAugItem))
+
+    def keep_ptr(self):
+        return self.keep.ctypes.data_as(C.c_void_p)
+
+
+def train_aug_batch(packed, train_size, device='cuda'):
+    """Apply a packed batch of plans on the GPU: one H2D copy of the uint8 buffer (asynchronous when the batch was
+    pinned by the DataLoader; no extra host copy is made here), one yb_train_aug launch.
+    Returns (images [B,3,S,S], targets: list of [n_i,5], masks: list of [n_i,S,S]), CUDA float32, the inputs
+    Yolact.forward(img, targets, masks) takes in train mode."""
+    S = int(train_size)
+    if S != packed.train_size:
+        raise ValueError(f'the plans were drawn for train_size {packed.train_size}, not {S}')
+    device = torch.device(device)
+    if device.type != 'cuda':
+        raise _lib.YolactB200Error('train_aug_batch runs on a CUDA device (no CPU fallback)')
+    B, G = len(packed), int(packed.keep.shape[0])
+    L = _lib.lib()
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream()
+        src = packed.buffer.to(device, non_blocking=packed.buffer.is_pinned())
+        ws_bytes = int(L.yb_train_aug_workspace_bytes(B, G))
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        images = torch.empty(B, 3, S, S, dtype=torch.float32, device=device)
+        masks = torch.empty(G, S, S, dtype=torch.float32, device=device)
+        _lib.check(L.yb_train_aug(src.data_ptr(), src.numel(), packed.items_ptr(), B, packed.keep_ptr(), S,
+                                  ws.data_ptr(), ws_bytes, images.data_ptr(), masks.data_ptr() if G else None, stream.cuda_stream),
+                   'yb_train_aug')
+        targets = [t.to(device, non_blocking=t.is_pinned()) for t in packed.targets]
+    return images, targets, list(masks.split(packed.num_keep, 0))
+
+
+class TrainAugLoader:
+    """Wraps a DataLoader whose collate is utils.coco.train_collate and yields what the reference's train loop
+    feeds the network (train.py:112-117), augmented on `device`:
+
+        for images, targets, masks in TrainAugLoader(data_loader, cfg.img_size):
+            loss_c, loss_b, loss_m, loss_s = net(images, targets, masks)
+    """
+
+    def __init__(self, loader, train_size, device=None):
+        self.loader, self.train_size = loader, int(train_size)
+        self.device = device if device is not None else torch.device('cuda', torch.cuda.current_device())
+
+    def __len__(self):
+        return len(self.loader)
+
+    def __iter__(self):
+        for packed in self.loader:
+            yield train_aug_batch(packed, self.train_size, self.device)
