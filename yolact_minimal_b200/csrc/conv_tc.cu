@@ -42,6 +42,7 @@
 #include <stdlib.h>
 #include <string.h>
 #include <mutex>
+#include <type_traits>
 
 namespace yb {
 
@@ -75,7 +76,37 @@ struct TcParams {
   const float* bias;
   int residual;           // out_mode 0: + the residual, loaded into the staging buffers by TMA (TcMaps::res)
   void* out;
+#ifdef YB_CONV_TRACE
+  unsigned long long* trace;
+#endif
 };
+
+// Trace build (tools/trace_conv.cu; the library never defines YB_CONV_TRACE): thread 0 of each consumer warpgroup writes
+// %globaltimer stamps for the launch that conv_trace_buf points at.  Per CTA (up to CT_TRACE_CTAS): trace[cta * 3] its start
+// (thread 0, before the barrier set-up), trace[cta * 3 + 1 + warpgroup] the warpgroup's exit (its stores complete).  Per tile, at
+// trace[CT_TRACE_CTAS * 3 + ((cta * 2 + warpgroup) * CT_TRACE_TILES + tile) * CT_TRACE_SLOTS + slot]: 0 k-loop start; 1 first
+// full-barrier wait done; 2 last MMA drained; 3 epilogue arithmetic done (the last segment staged); 4 last store issued.
+#ifdef YB_CONV_TRACE
+constexpr int CT_TRACE_CTAS = 1024, CT_TRACE_TILES = 96, CT_TRACE_SLOTS = 5;
+unsigned long long* conv_trace_buf = nullptr;
+__device__ __forceinline__ unsigned long long ct_now() {
+  unsigned long long ns;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
+  return ns;
+}
+#define CT_TRACE(slot)                                                                                                     \
+  do {                                                                                                                     \
+    if (p.trace && t == 0 && i < CT_TRACE_TILES)                                                                           \
+      p.trace[CT_TRACE_CTAS * 3 + (((size_t)blockIdx.x * 2 + c) * CT_TRACE_TILES + i) * CT_TRACE_SLOTS + (slot)] = ct_now(); \
+  } while (0)
+#define CT_TRACE_CTA(k)                                                                                                    \
+  do {                                                                                                                     \
+    if (p.trace) p.trace[(size_t)blockIdx.x * 3 + (k)] = ct_now();                                                        \
+  } while (0)
+#else
+#define CT_TRACE(slot) do { } while (0)
+#define CT_TRACE_CTA(k) do { } while (0)
+#endif
 
 // the staged epilogue's TMA maps, one per segment width (index 0: 64, 1: 32, 2: 16 columns; unused widths hold a placeholder)
 struct TcMaps {
@@ -280,6 +311,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
   const int wg = threadIdx.x >> 7;
   const uint32_t rank = p.pair ? cluster_ctarank() : 0u;
   if (threadIdx.x == 0) {
+    CT_TRACE_CTA(0);
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     // empty: one arrive per consumer warp -- of both CTAs in the pair form, whose weight half lands in both shared memories
@@ -359,8 +391,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
       kb_range(p, i, kb0, kb1);
       const int nmain = kb1 - kb0;
       int prev = -1;
+      CT_TRACE(0);
       for (int s = 0; s < nmain; ++s) {
         mbar_wait(&full[stage], phase);
+        if (s == 0) CT_TRACE(1);
         const uint64_t da = gmma_desc(smem_u32(sA + (size_t)stage * TC_A_STAGE + (size_t)c * (TC_A_STAGE / 2)));
         const uint32_t b_addr = smem_u32(sB + (size_t)stage * B_STAGE);
         const uint64_t db = MNB ? gmma_desc_mn(b_addr) : gmma_desc(b_addr);
@@ -380,6 +414,7 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
       wgmma_wait<0>();
       acc_fence<BN / 2>(acc);
       if (prev >= 0) release(prev);
+      CT_TRACE(2);
 
       // ---- epilogue: this thread's fragment holds rows r and r + 8 of the warpgroup's 64, columns 8j + 2 (lane % 4) + {0, 1} ----
       const int n0 = n_tile * BN;                                  // gemm: N tile n of tap t is column t * Nper + (n % gemm_ntile_tap) * BN
@@ -412,31 +447,36 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           }
         }
         const float2* bias = reinterpret_cast<const float2*>(p.bias + n0) + (lane & 3);
+        // the loop for one activation and residual setting (compile-time ACT / RES): the per-value arithmetic is straight-line code
+        auto stage_tile = [&](auto act_c, auto res_c) {
+          constexpr int ACT = decltype(act_c)::value;
+          constexpr bool RES = decltype(res_c)::value;
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {                         // j is a compile-time index: the segment arithmetic folds away
           const int s = Segs16<BN>::of(8 * j), w = Segs16<BN>::width(s), sb = Segs16<BN>::base(s);
           uint8_t* buf = stg + (q & 1) * TC_STG_BYTES;
-          if (p.residual && 8 * j == sb) mbar_wait(&res_full[2 * c + (q & 1)], (q >> 1) & 1);
+          if (RES && 8 * j == sb) mbar_wait(&res_full[2 * c + (q & 1)], (q >> 1) & 1);
           const float2 b = __ldg(bias + 4 * j);
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const uint32_t a = smem_u32(buf) + stg_off16(r0 + 8 * h, 8 * j - sb + 2 * (lane & 3), w);
             float v0 = b.x + acc[4 * j + 2 * h], v1 = b.y + acc[4 * j + 2 * h + 1];
-            if (p.residual) {
+            if (RES) {
               const float2 rr = unpack2<F16>(lds32(a));
               v0 += rr.x; v1 += rr.y;
             }
-            const uint32_t pk = pack2<F16>(apply_act(v0, p.relu), apply_act(v1, p.relu));
+            const uint32_t pk = pack2<F16>(apply_act(v0, ACT), apply_act(v1, ACT));
             sts32(a, zero[h] ? 0u : pk);
           }
           if (8 * j + 8 == sb + w) {                               // the segment is complete
+            if (8 * j + 8 == BN) CT_TRACE(3);
             fence_async_smem();
             if (t == 0) bulk_wait_read0();                         // the previous segment's store has read the other buffer
             named_barrier_sync(1 + c, 128);
             if (t == 0) {
               tma_store_2d(&maps.out[seg_map(w)], buf, n0 + sb, row0);
               bulk_commit();
-              if (p.residual) {                                    // the next segment's residual box, into the other buffer
+              if (RES) {                                           // the next segment's residual box, into the other buffer
                 int mt, nt;
                 if (s + 1 < Segs16<BN>::count) load_res(q + 1, m_tile, n_tile, s + 1);
                 else if (tile_at(p, i + 1, mt, nt)) load_res(q + 1, mt, nt, 0);
@@ -444,6 +484,17 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             }
             ++q;
           }
+        }
+        };
+        using F = std::false_type;
+        using T = std::true_type;
+        using A0 = std::integral_constant<int, 0>;
+        using A1 = std::integral_constant<int, 1>;
+        using A2 = std::integral_constant<int, 2>;
+        if (p.residual) {
+          if (p.relu == 1) stage_tile(A1{}, T{}); else if (p.relu == 2) stage_tile(A2{}, T{}); else stage_tile(A0{}, T{});
+        } else {
+          if (p.relu == 1) stage_tile(A1{}, F{}); else if (p.relu == 2) stage_tile(A2{}, F{}); else stage_tile(A0{}, F{});
         }
       } else {
         // ---- dense fp32 rows (halo rows skipped): staged per segment, copied out with 16-byte stores ----
@@ -462,6 +513,8 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           }
         }
         const float2* bias = reinterpret_cast<const float2*>(p.bias + n0) + (lane & 3);
+        auto stage_tile = [&](auto act_c) {                        // as above: one loop per activation
+          constexpr int ACT = decltype(act_c)::value;
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
           const int sb = (8 * j) / 32 * 32, w = BN - sb < 32 ? BN - sb : 32;
@@ -469,9 +522,10 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
           const float2 b = __ldg(bias + 4 * j);
 #pragma unroll
           for (int h = 0; h < 2; ++h)
-            sts64(buf + stg_off32(r0 + 8 * h, 8 * j - sb + 2 * (lane & 3)), apply_act(b.x + acc[4 * j + 2 * h], p.relu),
-                  apply_act(b.y + acc[4 * j + 2 * h + 1], p.relu));
+            sts64(buf + stg_off32(r0 + 8 * h, 8 * j - sb + 2 * (lane & 3)), apply_act(b.x + acc[4 * j + 2 * h], ACT),
+                  apply_act(b.y + acc[4 * j + 2 * h + 1], ACT));
           if (8 * j + 8 == sb + w) {
+            if (8 * j + 8 == BN) CT_TRACE(3);
             // every thread has staged this segment and finished copying out the previous one from the other buffer
             named_barrier_sync(1 + c, 128);
             const int ch = t & 7;
@@ -484,9 +538,15 @@ k_conv_tc(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUten
             ++q;
           }
         }
+        };
+        if (p.relu == 1) stage_tile(std::integral_constant<int, 1>{});
+        else if (p.relu == 2) stage_tile(std::integral_constant<int, 2>{});
+        else stage_tile(std::integral_constant<int, 0>{});
       }
+      CT_TRACE(4);                                                 // 16-bit: after the last segment's TMA store was issued
     }
     if (!MNB && t == 0) bulk_wait0();                              // the TMA stores are complete before the CTA exits
+    if (t == 0) CT_TRACE_CTA(1 + c);
   }
   if (p.pair) cluster_sync_all();                                  // neither CTA leaves while the peer may still signal its barriers
 }
@@ -989,6 +1049,9 @@ int launch_conv_tc(const TcPlan* pl, const ConvArgs& a, cudaStream_t s) {
   p.g = a.g; p.bias = a.bias; p.out = a.out;
   p.residual = a.residual != nullptr;
   p.gemm = 0; p.gemm_ntile_tap = 1; p.gemm_splits = 1;
+#ifdef YB_CONV_TRACE
+  p.trace = conv_trace_buf;
+#endif
   const int total = p.m_tiles * p.n_tiles;
   const int max_units = pl->pair ? pl->sms / 2 : pl->sms;
   const int units = total < max_units ? total : max_units;
