@@ -112,6 +112,23 @@ YB_API int yb_mask_assemble(const float* proto, const float* coef, const float* 
                      void* workspace, size_t workspace_bytes,
                      void* out_mask, int32_t* out_box_px, void* stream);
 
+/* Batched mask assembly, bit-packed output (mask_f32 = 2 above) -- after_nms for the detect_batched record of B images of any
+ * sizes, with no host sync on the detection counts.
+ *   proto [B,P,P,K] (Yolact.forward's proto), coef [B,D,K], box [B,D,4], count [B] int32: detect_batched's record (DEVICE).
+ *   img_hw [B,2] int32 (h, w) and mask_off [B+1] int64 are HOST tables: image b writes its masks [D,h_b,ceil(w_b/32)] words from
+ *   out_mask + mask_off[b]; it owns D*h_b*ceil(w_b/32) words there, which must end at or before mask_off[b+1], and mask_off[B] <=
+ *   mask_words.  Detections at or past count[b] write no mask words; their blocks exit at once.  out_box_px [B,D,4] int32 gets
+ *   every row: trunc(box * max(h_b,w_b)) below count[b], zero at or past it.
+ *   Image b's first count[b] masks and boxes equal yb_mask_assemble(mask_f32 = 2) on that image bit for bit.
+ * Every size and offset is checked on the host before anything is launched (YB_ERR_INVALID); the geometry table is then copied
+ * through library-owned page-locked staging (as yb_train_aug's), so the call queues without waiting for the stream.
+ * workspace: B*D*P*P floats plus the table (yb_mask_assemble_batch_workspace_bytes) -- 487 MB at B = 64, D = 100, P = 138. */
+YB_API size_t yb_mask_assemble_batch_workspace_bytes(int batch, int max_det, int proto_size);
+YB_API int yb_mask_assemble_batch(const float* proto, const float* coef, const float* box, const int32_t* count, int batch, int max_det,
+                                  int proto_size, int coef_dim, const int32_t* img_hw, const int64_t* mask_off, int64_t mask_words,
+                                  int crop, void* workspace, size_t workspace_bytes, uint32_t* out_mask, int32_t* out_box_px,
+                                  void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Mask output stage (SURVEY.md 8(f) rank 2) -- what the reference's evaluation loop does with the masks after after_nms:
  *   yb_pack_mask_bits   {0,1} masks [n,h,w] (uint8, or float32 when is_f32) -> packed words [n,h,ceil(w/32)]
@@ -180,6 +197,19 @@ YB_API int yb_eval_ap(const yb_eval_params* p, const float* rec_score, const int
  * top-left with the BGR mean, bilinear resize (OpenCV INTER_LINEAR coordinates), (x-mean)/std.
  * ---------------------------------------------------------------------------------------- */
 YB_API int yb_val_aug(const uint8_t* img_bgr, int h, int w, int img_size, float* out, void* stream);
+
+/* Batched form: src is one device buffer holding B uint8 BGR HWC images of any sizes; items is a HOST table, item i is the
+ * image [h,w,3] at byte img_off of src and writes out[i] ([B,3,S,S] float32 RGB).  One launch; image i equals yb_val_aug on it
+ * bit for bit.  Every offset and size is checked on the host before the launch (YB_ERR_INVALID); the table is then copied into
+ * the workspace through the page-locked staging of yb_train_aug, so the call queues without waiting for the stream. */
+typedef struct {
+  int64_t img_off;           /* byte offset of the image in src */
+  int32_t h, w;
+} yb_val_aug_item;
+
+YB_API size_t yb_val_aug_batch_workspace_bytes(int n_items);
+YB_API int yb_val_aug_batch(const uint8_t* src, int64_t src_bytes, const yb_val_aug_item* items, int n_items, int img_size,
+                            void* workspace, size_t workspace_bytes, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Training augmentation -- the pixel work of utils/augmentations.py:230-252 train_aug for a batch, given the

@@ -70,6 +70,11 @@ class TrainAugItem(C.Structure):
                                          'train_x', 'train_y', 'mask_u8', 'out_mask', 'keep_begin', 'num_keep')]
 
 
+class ValAugItem(C.Structure):
+    """yb_val_aug_item: where one image of a yb_val_aug_batch buffer lies."""
+    _fields_ = [('img_off', C.c_int64), ('h', C.c_int32), ('w', C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol declared in include/yolact_b200.h
 PROTOTYPES = {
     'yb_version': (C.c_int, []),
@@ -86,7 +91,12 @@ PROTOTYPES = {
     'yb_mask_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int]),
     'yb_mask_assemble': (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                    vp, C.c_size_t, vp, vp, vp]),
+    'yb_mask_assemble_batch_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    'yb_mask_assemble_batch': (C.c_int, [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, C.c_int64, C.c_int,
+                                         vp, C.c_size_t, vp, vp, vp]),
     'yb_val_aug': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp]),
+    'yb_val_aug_batch_workspace_bytes': (C.c_size_t, [C.c_int]),
+    'yb_val_aug_batch': (C.c_int, [vp, C.c_int64, vp, C.c_int, C.c_int, vp, C.c_size_t, vp, vp]),
     'yb_train_aug_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int64]),
     'yb_train_aug': (C.c_int, [vp, C.c_int64, C.POINTER(TrainAugItem), C.c_int, vp, C.c_int, vp, C.c_size_t, vp, vp, vp]),
     'yb_pack_mask_bits': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),

@@ -14,8 +14,6 @@
 #include "common.cuh"
 #include <float.h>
 #include <math.h>
-#include <string.h>
-#include <mutex>
 
 namespace yb {
 
@@ -192,53 +190,6 @@ __global__ void __launch_bounds__(kAugThreads) k_train_aug(const uint8_t* __rest
 
 namespace {
 size_t aug_items_bytes(int n_items) { return yb::align_up((size_t)n_items * sizeof(yb_train_aug_item), 256); }
-
-// Page-locked staging for the item and keep tables.  A copy from pageable memory may wait for the work already queued
-// on the stream; from page-locked memory it is queued like a kernel, so the host can submit batches ahead of training.
-// A slot is reused only after the copy that last read it has run; with kStagingSlots slots the host blocks only when it
-// is that many calls ahead of the stream.
-struct StagingSlot {
-  void* host = nullptr;
-  size_t cap = 0;
-  cudaEvent_t done = nullptr;
-  int device = -1;
-};
-constexpr int kStagingSlots = 4;
-std::mutex g_staging_mu;
-StagingSlot g_staging[kStagingSlots];
-int g_staging_next = 0;
-
-int stage_tables(const yb_train_aug_item* items, int n_items, const int32_t* keep, int64_t n_keep, void* workspace, cudaStream_t st) {
-  const size_t head = aug_items_bytes(n_items), bytes = head + (size_t)n_keep * sizeof(int32_t);
-  int device = 0;
-  YB_CHECK_CUDA(cudaGetDevice(&device));
-  std::lock_guard<std::mutex> lock(g_staging_mu);
-  StagingSlot& s = g_staging[g_staging_next];
-  g_staging_next = (g_staging_next + 1) % kStagingSlots;
-  if (s.done) {
-    YB_CHECK_CUDA(cudaEventSynchronize(s.done));
-    if (s.device != device) {
-      YB_CHECK_CUDA(cudaEventDestroy(s.done));
-      s.done = nullptr;
-    }
-  }
-  if (!s.done) {
-    YB_CHECK_CUDA(cudaEventCreateWithFlags(&s.done, cudaEventDisableTiming));
-    s.device = device;
-  }
-  if (s.cap < bytes) {
-    if (s.host) YB_CHECK_CUDA(cudaFreeHost(s.host));
-    s.host = nullptr;
-    s.cap = 0;
-    YB_CHECK_CUDA(cudaHostAlloc(&s.host, bytes, cudaHostAllocPortable));
-    s.cap = bytes;
-  }
-  memcpy(s.host, items, (size_t)n_items * sizeof(yb_train_aug_item));
-  if (n_keep) memcpy((char*)s.host + head, keep, (size_t)n_keep * sizeof(int32_t));
-  YB_CHECK_CUDA(cudaMemcpyAsync(workspace, s.host, bytes, cudaMemcpyHostToDevice, st));
-  YB_CHECK_CUDA(cudaEventRecord(s.done, st));
-  return YB_OK;
-}
 }  // namespace
 
 extern "C" size_t yb_train_aug_workspace_bytes(int n_items, int64_t n_keep) {
@@ -292,7 +243,9 @@ extern "C" int yb_train_aug(const uint8_t* src, int64_t src_bytes, const yb_trai
   cudaStream_t st = (cudaStream_t)stream;
   yb_train_aug_item* d_items = (yb_train_aug_item*)workspace;
   int32_t* d_keep = (int32_t*)((char*)workspace + aug_items_bytes(n_items));
-  YB_PROPAGATE(stage_tables(items, n_items, keep, n_keep, workspace, st));
+  const yb::StagePart parts[2] = {{items, (size_t)n_items * sizeof(yb_train_aug_item), 0},
+                                   {keep, (size_t)n_keep * sizeof(int32_t), aug_items_bytes(n_items)}};
+  YB_PROPAGATE(yb::stage_tables(workspace, aug_items_bytes(n_items) + (size_t)n_keep * sizeof(int32_t), parts, 2, st));
   dim3 grid(yb::ceil_div(S * S, yb::kAugThreads), n_items);
   yb::k_train_aug<<<grid, yb::kAugThreads, 0, st>>>(src, d_items, d_keep, S, out_img, out_masks);
   YB_CHECK_LAUNCH();

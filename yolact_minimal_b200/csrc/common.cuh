@@ -55,6 +55,19 @@ constexpr int kSmCount = 132;
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// ---- page-locked staging of host tables --------------------------------------------------------
+// Copies host tables into device memory on `st` through a small ring of library-owned page-locked slots.  A copy from
+// pageable memory may wait for the work already queued on the stream; from page-locked memory it is queued like a kernel,
+// so a caller can submit batches ahead of the device.  A slot is reused only after the copy that last read it has run, so
+// the host blocks only when it is a whole ring of calls ahead of the stream.  The caller's tables may be freed on return.
+// Part i is written at byte parts[i].offset of the `bytes` copied to device_dst.
+struct StagePart {
+  const void* src;
+  size_t bytes;
+  size_t offset;
+};
+int stage_tables(void* device_dst, size_t bytes, const StagePart* parts, int n_parts, cudaStream_t st);
+
 // ---- device helpers --------------------------------------------------------------------------
 #ifdef __CUDACC__
 __device__ __forceinline__ uint32_t float_to_ordered(float f) {

@@ -4,6 +4,9 @@
 yb_val_aug (one fused kernel: pad-to-square with the BGR mean, bilinear resize, normalise,
 BGR->RGB, HWC->CHW).  Takes the uint8 BGR image (numpy HWC, as cv2.imread returns it, or a CUDA
 uint8 tensor) and returns a CUDA float32 tensor [3, val_size, val_size].
+`val_aug_batch` does the same for a batch of images of any sizes packed in one buffer
+(`pack_images`, `PackedValBatch`), in one yb_val_aug_batch launch; image b of its output equals
+`val_aug` on image b bit for bit.
 
 `train_aug` (:230-252) is split in two.  Every random draw it makes depends only on shapes, boxes
 and labels, never on pixel values, so `train_aug_plan` replays those draws on the host (the same
@@ -36,6 +39,88 @@ def val_aug(img, val_size, device='cuda'):
         _lib.check(_lib.lib().yb_val_aug(img.data_ptr(), h, w, int(val_size), out.data_ptr(),
                                          torch.cuda.current_stream().cuda_stream), 'yb_val_aug')
     return out
+
+
+VAL_ITEM_DTYPE = np.dtype(_lib.ValAugItem)
+
+
+def pack_images(images):
+    """uint8 BGR images [h,w,3] of any sizes -> (torch uint8 buffer holding them back to back, numpy item table with
+    yb_val_aug_item's layout)."""
+    items = np.zeros(len(images), dtype=VAL_ITEM_DTYPE)
+    buf = np.empty(sum(im.nbytes for im in images), dtype=np.uint8)
+    off = 0
+    for i, im in enumerate(images):
+        if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
+            raise ValueError(f'image {i}: expected a uint8 HxWx3 BGR image, got {im.dtype} {im.shape}')
+        buf[off:off + im.nbytes] = im.reshape(-1)
+        items[i] = (off, im.shape[0], im.shape[1])
+        off += im.nbytes
+    return torch.from_numpy(buf), items
+
+
+def val_aug_batch(buffer, items, val_size, device='cuda'):
+    """val_aug for a batch: `buffer` a torch uint8 tensor holding B BGR HWC images back to back, `items` their numpy table
+    (pack_images).  One H2D copy of the buffer (asynchronous when it is pinned), one yb_val_aug_batch launch.
+    Returns a CUDA float32 tensor [B, 3, val_size, val_size]."""
+    device = torch.device(device)
+    if device.type != 'cuda':
+        raise _lib.YolactB200Error('val_aug_batch runs on a CUDA device (no CPU fallback)')
+    if not (isinstance(buffer, torch.Tensor) and buffer.dtype == torch.uint8 and buffer.dim() == 1):
+        raise ValueError('buffer must be a 1-D torch uint8 tensor')
+    items = np.ascontiguousarray(items, dtype=VAL_ITEM_DTYPE)
+    B, S = len(items), int(val_size)
+    L = _lib.lib()
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream()
+        src = buffer.to(device, non_blocking=buffer.is_pinned())
+        ws_bytes = int(L.yb_val_aug_batch_workspace_bytes(B))
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=device)
+        out = torch.empty(B, 3, S, S, dtype=torch.float32, device=device)
+        _lib.check(L.yb_val_aug_batch(src.data_ptr(), src.numel(), items.ctypes.data, B, S, ws.data_ptr(), ws_bytes, out.data_ptr(),
+                                      stream.cuda_stream), 'yb_val_aug_batch')
+    return out
+
+
+class PackedValBatch:
+    """A batch of validation images ready for val_aug_batch, with what MapEvaluator.add needs of their annotations:
+      buffer / items   the raw uint8 BGR images back to back and their yb_val_aug_item table (pack_images)
+      gt               torch float32 [G,5]: x1,y1,x2,y2 in [0,1] and the class, all images back to back; gt_offset [B+1]
+      gt_masks         torch int32: every image's packed gt masks [g_b, h_b, ceil(w_b/32)] back to back; gt_mask_off [B+1] (words)
+      sizes, ids       (h, w) and the COCO image id of every image
+    It is built in DataLoader workers (utils.coco.val_collate) and holds only picklable types; with DataLoader(pin_memory=True)
+    the loader's pin thread calls pin_memory() and the copies to the device are asynchronous."""
+
+    def __init__(self, samples):
+        """samples: list of (img_u8 [h,w,3], gt float32 [g,5], gt_bits int32 [g,h,ceil(w/32)], (h, w), image id)."""
+        self.buffer, self.items = pack_images([s[0] for s in samples])
+        self.sizes = [(int(s[3][0]), int(s[3][1])) for s in samples]
+        self.ids = [s[4] for s in samples]
+        for i, (img, gt, bits, (h, w), _) in enumerate(samples):
+            if img.shape[:2] != (h, w) or gt.dtype != np.float32 or gt.ndim != 2 or gt.shape[1] != 5 or bits.dtype != np.int32 or \
+                    bits.shape != (gt.shape[0], h, (w + 31) // 32):
+                raise ValueError(f'sample {i}: image {img.shape}, gt {gt.dtype} {gt.shape} and gt masks {bits.dtype} {bits.shape} do not '
+                                 f'describe one {h}x{w} image')
+        self.gt_offset = np.concatenate([[0], np.cumsum([s[1].shape[0] for s in samples])]).astype(int).tolist()
+        self.gt_mask_off = np.concatenate([[0], np.cumsum([s[2].size for s in samples])]).astype(int).tolist()
+        self.gt = torch.from_numpy(np.concatenate([s[1] for s in samples]).reshape(-1, 5))
+        self.gt_masks = torch.from_numpy(np.concatenate([s[2].reshape(-1) for s in samples]))
+
+    def __len__(self):
+        return len(self.items)
+
+    def pin_memory(self):
+        """Called by DataLoader(pin_memory=True) in its pin thread: page-locks the images, the gts and the gt masks."""
+        self.buffer, self.gt, self.gt_masks = self.buffer.pin_memory(), self.gt.pin_memory(), self.gt_masks.pin_memory()
+        return self
+
+    def gt_to(self, device):
+        """-> (gt [G,5], list of B packed gt masks [g_b, h_b, ceil(w_b/32)]) on `device`: views of one copy of each buffer."""
+        gt = self.gt.to(device, non_blocking=self.gt.is_pinned())
+        words = self.gt_masks.to(device, non_blocking=self.gt_masks.is_pinned())
+        o, g = self.gt_mask_off, self.gt_offset
+        masks = [words[o[b]:o[b + 1]].view(g[b + 1] - g[b], h, (w + 31) // 32) for b, (h, w) in enumerate(self.sizes)]
+        return gt, masks
 
 
 # ----------------------------------------------------------------------------- train_aug: host planner

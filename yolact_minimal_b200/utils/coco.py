@@ -1,16 +1,28 @@
-"""COCO training data for the GPU augmentation: the reference's utils/coco.py:47-133 COCODetection in 'train'
-mode and its train_collate (:14-28), with train_aug's pixel work left to the GPU.
+"""COCO data for the GPU augmentations: the reference's utils/coco.py:47-133 COCODetection and its collates.
 
-Each worker reads the image and decodes the instance masks as the reference does, applies the same annotation
-rules, and draws the train_aug plan on the host (utils.augmentations.train_aug_plan); it returns the raw uint8
-image, the raw uint8 masks and the plan.  train_collate packs a batch into one uint8 buffer plus the kernel's
-tables, and utils.augmentations.TrainAugLoader (or train_aug_batch) augments it on the device.
+'train' (COCODetection, train_collate :14-28): each worker reads the image and decodes the instance masks as the
+reference does, applies the same annotation rules, and draws the train_aug plan on the host
+(utils.augmentations.train_aug_plan); it returns the raw uint8 image, the raw uint8 masks and the plan.  train_collate
+packs a batch into one uint8 buffer plus the kernel's tables, and utils.augmentations.TrainAugLoader (or
+train_aug_batch) augments it on the device.
+
+'val' (COCOValDetection, val_collate :31-35): each worker returns the raw uint8 image, the gts and the gt masks
+bit-packed on the host; val_collate packs a batch into a PackedValBatch, and yolact_minimal_b200.eval.evaluate runs
+val_aug on the device for the whole batch (utils.augmentations.val_aug_batch).
 """
 import os.path as osp
 
 import numpy as np
 
-from .augmentations import PackedTrainBatch, train_aug_plan
+from .augmentations import PackedTrainBatch, PackedValBatch, train_aug_plan
+from .mask_utils import pack_masks_host
+
+
+def _imread(image_path, file_name):
+    import cv2
+    img_path = osp.join(image_path, file_name)
+    assert osp.exists(img_path), f'Image path does not exist: {img_path}'
+    return cv2.imread(img_path)
 
 
 def train_collate(batch):
@@ -45,10 +57,7 @@ class COCODetection:
         return len(self.ids)
 
     def load_image(self, file_name):
-        import cv2
-        img_path = osp.join(self.image_path, file_name)
-        assert osp.exists(img_path), f'Image path does not exist: {img_path}'
-        return cv2.imread(img_path)
+        return _imread(self.image_path, file_name)
 
     def __getitem__(self, index):
         img_id = self.ids[index]
@@ -73,3 +82,50 @@ class COCODetection:
         if plan is None:
             return None
         return np.ascontiguousarray(img), masks, plan
+
+
+def val_collate(batch):
+    """Packs a batch of COCOValDetection samples for val_aug_batch and MapEvaluator.add."""
+    return PackedValBatch(batch)
+
+
+class COCOValDetection:
+    """The reference's COCODetection(cfg, mode='val') for batched evaluation on the GPU.  Its annotation rules
+    (utils/coco.py:69-119): crowd annotations are dropped, no box is filtered out, labels are continuous_id - 1, gt boxes
+    are divided by (w, h, w, h) in float64 and then rounded to float32 (as val_collate's torch.tensor does); an image with no
+    annotation left raises RuntimeError.  len() honours cfg.val_num.
+
+    Returns (img_u8 [h,w,3] BGR, gt float32 [n,5], gt masks bit-packed int32 [n,h,ceil(w/32)] (mask_utils.pack_masks layout),
+    (h, w), COCO image id); val_aug runs on the device for a whole batch.  `coco` may be passed in (any object with the
+    pycocotools.coco.COCO methods used here); by default it is pycocotools' COCO on cfg.val_ann."""
+
+    def __init__(self, cfg, coco=None):
+        self.cfg = cfg
+        self.image_path = cfg.val_imgs
+        if coco is None:
+            from pycocotools.coco import COCO
+            coco = COCO(cfg.val_ann)
+        self.coco = coco
+        self.ids = list(self.coco.imgToAnns.keys())
+        self.continuous_id = cfg.continuous_id
+
+    def __len__(self):
+        return len(self.ids) if self.cfg.val_num == -1 else min(self.cfg.val_num, len(self.ids))
+
+    def load_image(self, file_name):
+        return _imread(self.image_path, file_name)
+
+    def __getitem__(self, index):
+        img_id = self.ids[index]
+        target = [a for a in self.coco.loadAnns(self.coco.getAnnIds(imgIds=img_id)) if not a['iscrowd']]
+        img = self.load_image(self.coco.loadImgs(img_id)[0]['file_name'])
+        height, width, _ = img.shape
+        if not target:
+            raise RuntimeError('Error, no valid object in this image.')
+        boxes = np.array([[a['bbox'][0], a['bbox'][1], a['bbox'][0] + a['bbox'][2], a['bbox'][1] + a['bbox'][3]] for a in target])
+        labels = np.array([self.continuous_id[a['category_id']] - 1 for a in target])
+        masks = np.stack([self.coco.annToMask(a) for a in target], axis=0)
+        assert masks.shape == (boxes.shape[0], height, width), 'Unmatched annotations.'
+        boxes = boxes / np.array([width, height, width, height])
+        gt = np.hstack((boxes, np.expand_dims(labels, axis=1))).astype(np.float32)
+        return np.ascontiguousarray(img), gt, pack_masks_host(masks), (height, width), img_id

@@ -104,7 +104,10 @@ class MakeJson:
                 raise _lib.YolactB200Error('MakeJson.add_mask encodes on a CUDA device (no CPU fallback)')
             seg = seg.cuda()
         h, w = seg.shape
-        rle = mask_utils.encode_rle(mask_utils.pack_masks(seg[None]), h, w)[0]
+        self.add_mask_rle(image_id, category_id, mask_utils.encode_rle(mask_utils.pack_masks(seg[None]), h, w)[0], score)
+
+    def add_mask_rle(self, image_id, category_id, rle, score):
+        """A mask record from its COCO RLE (mask_utils.encode_rle of packed masks)."""
         self.mask_data.append({'image_id': int(image_id), 'category_id': self.coco_cats[int(category_id)], 'segmentation': rle,
                                'score': float(score)})
 

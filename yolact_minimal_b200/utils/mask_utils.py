@@ -35,6 +35,16 @@ def pack_masks(masks):
     return out
 
 
+def pack_masks_host(masks):
+    """pack_masks on the host: {0,1} masks [n,h,w] (numpy) -> numpy int32 words [n,h,ceil(w/32)] in the same layout
+    (np.packbits with little bit order over rows padded to 32 pixels; 8x less to pickle and copy than the uint8 masks)."""
+    m = np.asarray(masks)
+    n, h, w = m.shape
+    rows = np.zeros((n, h, (w + 31) // 32 * 32), np.uint8)
+    rows[..., :w] = m
+    return np.ascontiguousarray(np.packbits(rows, axis=-1, bitorder='little')).view('<i4')
+
+
 def unpack_masks(bits, w):
     """Packed words [n,h,words] -> uint8 masks [n,h,w] (plain torch bit arithmetic; for tests and visualisation)."""
     n, h, words = bits.shape

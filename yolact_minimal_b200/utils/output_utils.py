@@ -1,9 +1,9 @@
 """Post-process API kept from the reference's utils/output_utils.py -- `nms` (:126-163),
 `after_nms` (:200-233) and `draw_img` (:308-369) -- with the work done by the CUDA kernels behind
 yb_detect / yb_mask_assemble / yb_draw_masks (include/yolact_b200.h).  Same arguments, same return
-tuples, same "(None, ...)" convention for "no detections".  `detect_batched` is the batched form the
-reference lacks (its nms() squeezes a batch of 1, output_utils.py:127-130); `blend_masks` is
-draw_img's overlay on device-resident frames.
+tuples, same "(None, ...)" convention for "no detections".  `detect_batched` and `after_nms_batched`
+are the batched forms the reference lacks (its nms() squeezes a batch of 1, output_utils.py:127-130);
+`blend_masks` is draw_img's overlay on device-resident frames.
 
 All inputs must be CUDA tensors (draw_img also takes numpy arrays, which it uploads); nothing here
 falls back to the CPU.
@@ -164,6 +164,40 @@ def after_nms(ids_p, class_p, box_p, coef_p, proto_p, img_h, img_w, cfg=None, im
                                       crop, fmt, ws.data_ptr(), ws.numel(), masks.data_ptr(),
                                       boxes_px.data_ptr(), torch.cuda.current_stream().cuda_stream), 'yb_mask_assemble')
     return ids_p, class_p, boxes_px, masks
+
+
+def after_nms_batched(det, proto, sizes, crop=True):
+    """after_nms for a whole detect_batched record, bit-packed masks, with no host sync on the counts (yb_mask_assemble_batch).
+    det: detect_batched's dict (count [B], box [B,D,4], coef [B,D,K]); proto [B,P,P,K] (Yolact.forward's proto); sizes: B (h, w).
+    Returns (boxes_px [B,D,4] int32: pixel boxes of max(h_b, w_b), zero at or past count[b]; a list of B packed-mask views
+    [D, h_b, ceil(w_b/32)] int32 into one buffer, of which the first count[b] masks are written) -- the boxes_px and masks
+    MapEvaluator.add takes.  Image b's first count[b] masks and boxes equal after_nms(..., mask_dtype='bits') on that image."""
+    import numpy as np
+    count, box, coef = det['count'], det['box'], det['coef']
+    _require_cuda(count, box, coef, proto)
+    dev = proto.device
+    B, D, K = coef.shape
+    proto = proto.detach().to(torch.float32).contiguous()
+    P = proto.shape[1]
+    if tuple(proto.shape) != (B, P, P, K) or tuple(box.shape) != (B, D, 4) or tuple(count.shape) != (B,):
+        raise ValueError(f'proto {tuple(proto.shape)}, box {tuple(box.shape)}, count {tuple(count.shape)} do not match coef {tuple(coef.shape)}')
+    hw = np.ascontiguousarray(np.asarray(sizes, dtype=np.int64).reshape(-1, 2))
+    if hw.shape[0] != B or (hw <= 0).any() or (hw > 65535).any():
+        raise ValueError(f'sizes must hold {B} (h, w) pairs in 1..65535, got {sizes}')
+    n_words = D * hw[:, 0] * ((hw[:, 1] + 31) // 32)
+    off = np.concatenate([[0], np.cumsum(n_words)]).astype(np.int64)
+    hw32 = hw.astype(np.int32)
+    count, box, coef = (t.to(dt).contiguous() for t, dt in ((count, torch.int32), (box, torch.float32), (coef, torch.float32)))
+    masks = torch.empty(int(off[-1]), dtype=torch.int32, device=dev)
+    boxes_px = torch.empty(B, D, 4, dtype=torch.int32, device=dev)
+    L = _lib.lib()
+    with torch.cuda.device(dev):
+        ws = torch.empty(int(L.yb_mask_assemble_batch_workspace_bytes(B, D, P)), dtype=torch.uint8, device=dev)
+        _lib.check(L.yb_mask_assemble_batch(proto.data_ptr(), coef.data_ptr(), box.data_ptr(), count.data_ptr(), B, D, P, K, hw32.ctypes.data, off.ctypes.data, masks.numel(), 1 if crop else 0, ws.data_ptr(),
+                                            ws.numel(), masks.data_ptr(), boxes_px.data_ptr(), torch.cuda.current_stream().cuda_stream),
+                   'yb_mask_assemble_batch')
+    views = [masks[int(off[b]):int(off[b + 1])].view(D, int(h), (int(w) + 31) // 32) for b, (h, w) in enumerate(hw)]
+    return boxes_px, views
 
 
 # ---------------------------------------------------------------------------------------------------------------------------
