@@ -23,38 +23,56 @@ def stage_inputs(g):
     return tg, mk, class_p, box_p, coef_p, proto_p, seg_p
 
 
-def run_native_losses(dev, cfg, anchors, tg, mk, class_p, box_p, coef_p, proto_p, seg_nchw, grads=True, grad_scale=None, seed=1):
-    """yb_losses through ctypes.  Returns dict(losses, labels, matched_idx, offsets, neg, d_cls, d_box, d_coef, d_proto, d_seg (NCHW))."""
+def run_native_losses(dev, cfg, anchors, tg, mk, class_p, box_p, coef_p, proto_p, seg_nchw, grads=True, grad_scale=None, seed=1,
+                      pos_iou_thr=None, neg_iou_thr=None, masks_to_train=None, ld_seg=None, sentinel=None, check=True):
+    """yb_losses through ctypes.  Returns dict(losses, labels, matched_idx, offsets, neg, d_cls, d_box, d_coef, d_proto, d_seg (NCHW)).
+    pos_iou_thr / neg_iou_thr / masks_to_train override cfg; the coefficient dimension is coef_p's last.  ld_seg > C-1 pads every
+    seg row with columns the kernels must neither read (they hold NaN) nor leave unwritten (d_seg_nhwc keeps them).  grad_scale is
+    passed in device memory.  sentinel: fill every output with this value before the call (integer outputs with int(sentinel)).
+    check=False returns dict(status=..., outputs) instead of raising when yb_losses refuses the call."""
     from yolact_minimal_b200 import _lib
     L = _lib.lib()
     t = lambda a, dt=torch.float32: torch.from_numpy(np.ascontiguousarray(a)).to(dev, dt)
     B, A, C = class_p.shape
     K, P, Hs, S = coef_p.shape[-1], proto_p.shape[1], seg_nchw.shape[-1], mk[0].shape[-1]
+    ld = C - 1 if ld_seg is None else ld_seg
     cls, box, coef, proto = t(class_p), t(box_p), t(coef_p), t(proto_p)
-    seg = t(seg_nchw).permute(0, 2, 3, 1).contiguous()                     # the engine's layout: NHWC, ld = C-1
-    gt = t(np.concatenate(tg)); masks = t(np.concatenate(mk))
+    seg = torch.full((B, Hs, Hs, ld), float('nan'), device=dev)            # the engine's layout: NHWC, row stride ld
+    seg[..., :C - 1] = t(seg_nchw).permute(0, 2, 3, 1)
+    gt = t(np.concatenate(tg).reshape(-1, 5)); masks = t(np.concatenate(mk))  # exactly total_gt rows
     counts = [len(x) for x in tg]
     gt_off = torch.tensor(np.concatenate([[0], np.cumsum(counts)]).astype(np.int32), device=dev)
-    p = _lib.LossParams(B, A, C, K, P, Hs, S, float(cfg.pos_iou_thre), float(cfg.neg_iou_thre), 3, int(cfg.masks_to_train), float(cfg.conf_alpha),
+    thr = lambda v, d: float(d if v is None else v)
+    p = _lib.LossParams(B, A, C, K, P, Hs, S, thr(pos_iou_thr, cfg.pos_iou_thre), thr(neg_iou_thr, cfg.neg_iou_thre), 3,
+                        int(cfg.masks_to_train if masks_to_train is None else masks_to_train), float(cfg.conf_alpha),
                         float(cfg.bbox_alpha), float(cfg.mask_alpha), float(cfg.semantic_alpha))
-    ws = torch.empty(int(L.yb_losses_workspace_bytes(ctypes.byref(p), int(gt.shape[0]))), dtype=torch.uint8, device=dev)
-    out = dict(losses=torch.zeros(4, device=dev), labels=torch.zeros(B, A, dtype=torch.int32, device=dev),
-               matched_idx=torch.zeros(B, A, dtype=torch.int32, device=dev), offsets=torch.zeros(B, A, 4, device=dev),
-               neg=torch.zeros(B, A, dtype=torch.uint8, device=dev))
+    ws = torch.empty(max(1, int(L.yb_losses_workspace_bytes(ctypes.byref(p), int(gt.shape[0])))), dtype=torch.uint8, device=dev)
+    fi = 0 if sentinel is None else int(sentinel)
+    out = dict(losses=torch.full((4,), 0.0 if sentinel is None else float(sentinel), device=dev),
+               labels=torch.full((B, A), fi, dtype=torch.int32, device=dev), matched_idx=torch.full((B, A), fi, dtype=torch.int32, device=dev),
+               offsets=torch.full((B, A, 4), 0.0 if sentinel is None else float(sentinel), device=dev),
+               neg=torch.full((B, A), fi & 255, dtype=torch.uint8, device=dev))
     if grads:
-        out.update(d_cls=torch.full_like(cls, 7.0), d_box=torch.full_like(box, 7.0), d_coef=torch.full_like(coef, 7.0), d_proto=torch.full_like(proto, 7.0),
-                   d_seg=torch.full_like(seg, 7.0))
+        fv = 7.0 if sentinel is None else float(sentinel)
+        out.update(d_cls=torch.full_like(cls, fv), d_box=torch.full_like(box, fv), d_coef=torch.full_like(coef, fv), d_proto=torch.full_like(proto, fv),
+                   d_seg=torch.full_like(seg, fv))
     ptr = lambda k: out[k].data_ptr() if k in out else None
     gs = None if grad_scale is None else t(np.asarray(grad_scale, np.float32))
-    _lib.check(L.yb_losses(ctypes.byref(p), cls.data_ptr(), box.data_ptr(), coef.data_ptr(), proto.data_ptr(), seg.data_ptr(), C - 1, t(anchors).data_ptr(),
-                           gt.data_ptr(), gt_off.data_ptr(), masks.data_ptr(), int(gt.shape[0]), max(counts), seed, None if gs is None else gs.data_ptr(),
-                           out['losses'].data_ptr(), ptr('d_cls'), ptr('d_box'), ptr('d_coef'), ptr('d_proto'), ptr('d_seg'), out['labels'].data_ptr(),
-                           out['matched_idx'].data_ptr(), out['offsets'].data_ptr(), out['neg'].data_ptr(), ws.data_ptr(), ws.numel(),
-                           torch.cuda.current_stream().cuda_stream), 'yb_losses')
+    status = L.yb_losses(ctypes.byref(p), cls.data_ptr(), box.data_ptr(), coef.data_ptr(), proto.data_ptr(), seg.data_ptr(), ld, t(anchors).data_ptr(),
+                         gt.data_ptr(), gt_off.data_ptr(), masks.data_ptr(), int(gt.shape[0]), max(counts), seed, None if gs is None else gs.data_ptr(),
+                         out['losses'].data_ptr(), ptr('d_cls'), ptr('d_box'), ptr('d_coef'), ptr('d_proto'), ptr('d_seg'), out['labels'].data_ptr(),
+                         out['matched_idx'].data_ptr(), out['offsets'].data_ptr(), out['neg'].data_ptr(), ws.data_ptr(), ws.numel(),
+                         torch.cuda.current_stream().cuda_stream)
+    if check:
+        _lib.check(status, 'yb_losses')
     torch.cuda.synchronize()
     if grads:
-        out['d_seg'] = out['d_seg'].permute(0, 3, 1, 2).contiguous()
-    return {k: v.cpu().numpy() for k, v in out.items()}
+        out['d_seg_nhwc'] = out['d_seg']
+        out['d_seg'] = out['d_seg'][..., :C - 1].permute(0, 3, 1, 2).contiguous()
+    res = {k: v.cpu().numpy() for k, v in out.items()}
+    if not check:
+        res['status'] = int(status)
+    return res
 
 
 def torch_losses_and_grads(cfg, anchors, tg, mk, class_p, box_p, coef_p, proto_p, seg_p, grad_scale=(1, 1, 1, 1)):

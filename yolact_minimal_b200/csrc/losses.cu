@@ -25,7 +25,7 @@ struct LossWs {                          // carved out of the caller's workspace
   int32_t* labels;        // [B,A]   >0 fg class+1, 0 bg, -1 neutral
   float* offsets;         // [B,A,4]
   float* matched;         // [B,A,4]
-  float* mark;            // [B,A]
+  uint32_t* mark;         // [B,A]   OHEM mark as an ascending key (float_to_ordered)
   uint8_t* neg;           // [B,A]
   int32_t* num_pos;       // [B] + total at [B]
   uint32_t* logit_max;    // [1] ordered-uint max of all class logits
@@ -114,12 +114,14 @@ __global__ void __launch_bounds__(256) k_match_finalize(const float* __restrict_
   for (int a = threadIdx.x; a < A; a += 256) {
     const size_t i = (size_t)b * A + a;
     const int j = best_gt[i];
-    const float* g = gt + (size_t)(g0 + j) * 5;
+    const float* g = gt + (size_t)(g0 + j) * 5;         // read only when n > 0: an empty last image's g0 is one row past the buffer
     const float iou = best_iou[i];
-    int lab = (int)g[4] + 1;
-    if (iou < pos_thr) lab = -1;
-    if (iou < neg_thr) lab = 0;
-    if (n == 0) lab = 0;
+    int lab = 0;
+    if (n > 0) {
+      lab = (int)g[4] + 1;
+      if (iou < pos_thr) lab = -1;
+      if (iou < neg_thr) lab = 0;
+    }
     labels[i] = lab;
     cnt += lab > 0;
     const float* an = anchors + (size_t)a * 4;
@@ -152,7 +154,7 @@ __global__ void __launch_bounds__(256) k_logit_max(const float* __restrict__ x, 
 }
 
 __global__ void __launch_bounds__(256) k_ohem_mark(const float* __restrict__ cls, const int32_t* __restrict__ labels, const uint32_t* __restrict__ logit_max,
-                                                   long long rows, int NC, float* __restrict__ mark) {
+                                                   long long rows, int NC, uint32_t* __restrict__ mark) {
   const int lane = threadIdx.x & 31;
   const long long r = blockIdx.x * 8LL + (threadIdx.x >> 5);
   if (r >= rows) return;
@@ -162,10 +164,12 @@ __global__ void __launch_bounds__(256) k_ohem_mark(const float* __restrict__ cls
   for (int c = lane; c < NC; c += 32) s += expf(x[c] - gm);
 #pragma unroll
   for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
-  if (lane == 0) mark[r] = labels[r] != 0 ? 0.f : (logf(s) + gm) - x[0];      // positives and neutrals are filtered out (:213-214)
+  // positives and neutrals are filtered out (:213-214).  The true mark is >= 0, but its fp32 value is not: when class 0 holds the
+  // row's maximum and gm is large, it rounds to -ulp(gm).  The ordered key sorts such a mark below the zeroed rows, as torch.sort does.
+  if (lane == 0) mark[r] = float_to_ordered(labels[r] != 0 ? 0.f : (logf(s) + gm) - x[0]);
 }
 
-// k-th largest of n non-negative floats (as uint32 keys) by 4 radix passes over shared histograms; returns the key value
+// k-th largest of n uint32 keys by 4 radix passes over shared histograms; returns the key value
 __device__ uint32_t block_kth_largest(const uint32_t* __restrict__ keys, int n, int k, uint32_t* hist /*[256]*/, uint32_t* bc /*[2]*/) {
   uint32_t prefix = 0, mask = 0;
   int remaining = k;
@@ -191,13 +195,13 @@ __device__ uint32_t block_kth_largest(const uint32_t* __restrict__ keys, int n, 
 
 // per image: the num_neg = min(3 * num_pos, A - 1) anchors with the largest marks; ties by ascending anchor index (a stable
 // descending sort, yolact.py:216-220); positives / neutrals are cleared afterwards (:223-224)
-__global__ void __launch_bounds__(1024) k_ohem_select(const float* __restrict__ mark, const int32_t* __restrict__ labels, const int32_t* __restrict__ num_pos,
+__global__ void __launch_bounds__(1024) k_ohem_select(const uint32_t* __restrict__ mark, const int32_t* __restrict__ labels, const int32_t* __restrict__ num_pos,
                                                       int A, int ratio, uint8_t* __restrict__ neg) {
   __shared__ uint32_t hist[256];
   __shared__ uint32_t bc[2];
   __shared__ int scan[1024];
   const int b = blockIdx.x;
-  const uint32_t* keys = reinterpret_cast<const uint32_t*>(mark + (size_t)b * A);
+  const uint32_t* keys = mark + (size_t)b * A;
   int k = ratio * num_pos[b];
   if (k > A - 1) k = A - 1;
   if (k <= 0) { for (int a = threadIdx.x; a < A; a += blockDim.x) neg[(size_t)b * A + a] = 0; return; }
@@ -416,7 +420,11 @@ __global__ void __launch_bounds__(kMaskPix) k_mask_loss(const float* __restrict_
       const float p = 1.f / (1.f + expf(-z));
       const float lp = fmaxf(logf(p), -100.f), lq = fmaxf(logf(1.f - p), -100.f);        // torch clamps the logs at -100
       loss += s_w[i] * -(t * lp + (1.f - t) * lq);
+      // torch's chain: BCE backward (p - t) / max(p (1 - p), 1e-12), then sigmoid backward * p (1 - p).  The two cancel unless the
+      // clamp bites: a saturated wrong prediction (p rounds to 0 or 1) then gets a vanishing gradient, as in the reference.
       g = s_w[i] * (p - t) * gscale;
+      const float pq = p * (1.f - p);
+      if (pq < 1e-12f) g = g / 1e-12f * pq;
 #pragma unroll
       for (int k = 0; k < 32; ++k) dp[k] = fmaf(g, s_coef[i * 32 + k], dp[k]);
     } else if (t > 0.f) {
@@ -499,7 +507,7 @@ size_t carve(LossWs* w, char* base, const yb_loss_params& p, int total_gt) {
   w->best_iou = (float*)take(BA * 4); w->best_gt = (int32_t*)take(BA * 4);
   w->gt_anchor = (int32_t*)take((size_t)p.batch * kMaxGt * 4);
   w->labels = (int32_t*)take(BA * 4); w->offsets = (float*)take(BA * 16); w->matched = (float*)take(BA * 16);
-  w->mark = (float*)take(BA * 4); w->neg = (uint8_t*)take(BA);
+  w->mark = (uint32_t*)take(BA * 4); w->neg = (uint8_t*)take(BA);
   w->num_pos = (int32_t*)take((size_t)(p.batch + 1) * 4); w->logit_max = (uint32_t*)take(4); w->acc = (double*)take(4 * 8);
   w->ds_mask = (uint8_t*)take((size_t)(total_gt > 0 ? total_gt : 1) * p.proto_size * p.proto_size);
   w->sel = (int32_t*)take((size_t)p.batch * p.masks_to_train * 4); w->sel_count = (int32_t*)take((size_t)p.batch * 2 * 4);
@@ -565,7 +573,7 @@ int losses_impl(const yb_loss_params* p, const float* cls, const float* box, con
     YB_CHECK_LAUNCH();
   }
   // the OHEM mark buffer is free again: reuse it for the random subset keys
-  k_mask_select<<<B, 1024, 0, s>>>(w.labels, A, p->masks_to_train, seed, seed_dev, reinterpret_cast<uint32_t*>(w.mark), w.sel, w.sel_count, B);
+  k_mask_select<<<B, 1024, 0, s>>>(w.labels, A, p->masks_to_train, seed, seed_dev, w.mark, w.sel, w.sel_count, B);
   YB_CHECK_LAUNCH();
   if (d_coef) YB_CHECK_CUDA(cudaMemsetAsync(d_coef, 0, (size_t)rows * K * 4, s));
   {
