@@ -451,7 +451,8 @@ YB_API int yb_losses(const yb_loss_params* p, const float* cls, const float* box
                      void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * Training engine: Yolact.forward in training mode (modules/yolact.py:141-161) and its backward pass, ResNet-50/101 backbones.
+ * Training engine: Yolact.forward in training mode (modules/yolact.py:141-161) and its backward pass, ResNet-50/101 and Swin-T
+ * (depth 0: no BatchNorm buffers; stochastic depth drawn on the device from `seed`) backbones.
  * Train-mode forward = wgmma convolutions on 16-bit activations + batch-statistics BatchNorm (running statistics updated in
  * place, momentum 0.1) + the loss kernels above; backward = dgrad convolutions and weight-gradient GEMMs on the same wgmma
  * kernel, BatchNorm / pooling / up-sampling backward on CUDA cores.  The fp32 master parameters stay where the caller keeps
@@ -480,7 +481,12 @@ YB_API int yb_train_forward(yb_train* t, const float* img, const float* gt, cons
                             int max_gt_per_image, const yb_train_hparams* hp, uint32_t seed, float* losses, void* stream);
 /* gradients of sum_i loss_grad[i] * losses[i] (loss_grad: 4 DEVICE floats, NULL = ones) into the bound gradient buffers (overwritten) */
 YB_API int yb_train_backward(yb_train* t, const float* loss_grad, void* stream);
-/* debug / parity taps: copy a named activation (grad = 0) or its gradient (grad = 1) as NCHW float32 [B,C,H,H] (device) */
+/* debug / parity taps: copy a named activation (grad = 0) or its gradient (grad = 1) as NCHW float32 [B,C,H,H] (device).
+ * Swin-T names: "patch_embed"; per block P = "backbone.layers.<s>.blocks.<b>": P".norm1", P".attn.qkv" (q | k | v, 3C channels),
+ * P".attn" (attention output), P".attn.proj", P".x1" (after the attention residual), P".norm2", P".mlp.fc1" (before GELU),
+ * P".mlp.gelu", P".mlp.fc2", P".out"; per merge D = "backbone.layers.<s>.downsample": D".merge" (gathered 4C tokens), D".norm",
+ * D".reduction"; "c3" / "c4" / "c5" (backbone.norm1..3).  "out.drop_path": the step's stochastic-depth masks [B,12,2] (block,
+ * attention | MLP), C = 2, H = 12, no gradient; the "out.*" network outputs likewise. */
 YB_API int yb_train_read(yb_train* t, const char* name, int grad, float* out, int64_t out_count, int* C, int* H, void* stream);
 YB_API uint64_t yb_train_launches_per_step(const yb_train* t);
 

@@ -988,7 +988,7 @@ static int launch(const TcPlan* pl, const TcParams& p, const TcMaps& maps, bool 
 // ---- plain GEMM over long K on the same kernel (weight gradients; see TcParams::gemm) ---------------------------
 int tc_plan_create_gemm(const GemmArgs& g, TcPlan** out) {
   YB_REQUIRE(g.act_dt == DT_BF16 || g.act_dt == DT_F16, YB_ERR_UNSUPPORTED, "tc_plan_create_gemm: 16-bit operands only");
-  YB_REQUIRE(g.M >= 1 && g.K >= 1 && g.lda % 8 == 0 && g.ldb % 8 == 0 && g.ldb >= g.Nper && g.ntaps >= 1 && g.ntaps <= 16, YB_ERR_INVALID,
+  YB_REQUIRE(g.M >= 1 && g.K >= 1 && g.lda % 8 == 0 && g.ldb % 8 == 0 && g.ldb > g.Nper - 64 && g.ntaps >= 1 && g.ntaps <= 16, YB_ERR_INVALID,
              "tc_plan_create_gemm: M=%d K=%d lda=%d ldb=%d ntaps=%d", g.M, g.K, g.lda, g.ldb, g.ntaps);
   int bn = 0;
   if (g.Nper % 256 == 0) bn = 256;
@@ -1000,8 +1000,10 @@ int tc_plan_create_gemm(const GemmArgs& g, TcPlan** out) {
   plan_stages(pl);
   const bool f16 = g.act_dt == DT_F16;
   int s = make_map(&pl->tmA, g.a, (uint64_t)g.K, (uint64_t)g.M, TC_BM, f16, TC_BK, (uint64_t)g.lda);
-  // B is read MN-major straight from the [Kb pixels][ldb channels] activations: boxes of [64 k-rows][64 channels]
-  if (s == YB_OK) s = make_map(&pl->tmB, g.b, (uint64_t)g.Nper, (uint64_t)g.Kb, 64, f16, TC_BK, (uint64_t)g.ldb);
+  // B is read MN-major straight from the [Kb pixels][ldb channels] activations: boxes of [64 k-rows][64 channels].  With fewer than
+  // Nper channels (ldb = 96, Nper = 128: Swin-T stage 1) the TMA zero-fills the last box's missing channels.
+  const uint64_t nb = (uint64_t)(g.ldb < g.Nper ? g.ldb : g.Nper);
+  if (s == YB_OK) s = make_map(&pl->tmB, g.b, nb, (uint64_t)g.Kb, 64, f16, TC_BK, (uint64_t)g.ldb);
   if (s == YB_OK) s = tc_device_setup(f16, true, bn, &pl->sms);
   if (s != YB_OK) { delete pl; return s; }
   *out = pl;

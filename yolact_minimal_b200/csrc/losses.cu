@@ -307,8 +307,6 @@ __global__ void __launch_bounds__(256) k_downsample_masks(const float* __restric
 }
 
 // ---- positives of an image, in anchor order; more than `limit` -> a uniformly random subset of `limit` (yolact.py:261-268) ----
-__device__ __forceinline__ uint32_t hash32(uint32_t x) { x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16; return x; }
-
 __global__ void __launch_bounds__(1024) k_mask_select(const int32_t* __restrict__ labels, int A, int limit, uint32_t seed_value, const uint32_t* __restrict__ seed_dev,
                                                       uint32_t* __restrict__ keys_ws /*[B,A]*/,
                                                       int32_t* __restrict__ sel, int32_t* __restrict__ sel_count, int B) {

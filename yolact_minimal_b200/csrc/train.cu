@@ -1,6 +1,7 @@
-// Training engine (SURVEY.md 8 row a12): Yolact.forward in training mode and its backward pass for the ResNet backbones,
-// restated as two flat launch lists over persistent buffers (modules/resnet.py:20-98, modules/yolact.py:12-161 forward;
-// the backward is derived here -- the reference gets it from torch autograd).
+// Training engine (SURVEY.md 8 row a12): Yolact.forward in training mode and its backward pass for the ResNet and Swin-T backbones,
+// restated as two flat launch lists over persistent buffers (modules/resnet.py:20-98, modules/swin_transformer.py:436-518,
+// modules/yolact.py:12-161 forward; the backward is derived here -- the reference gets it from torch autograd).  Swin-T's linear
+// layers are 1x1 convs on the kernels below; its LayerNorm / attention / GELU / merge / stochastic-depth kernels are swin_train.cu.
 //
 //   forward   conv (wgmma, 16-bit operands, fp32 accumulate, raw output) -> batch statistics -> affine + ReLU (+ residual);
 //             FPN / ProtoNet / heads as in inference but with raw logits; targets + the four losses (losses.cu)
@@ -87,6 +88,7 @@ struct yb_train {
   PackDesc* d_pack = nullptr; UnpackDesc* d_unpack = nullptr;
   float* stats = nullptr; size_t stats_floats = 0, stats_cap = 0;    // zeroed at the start of forward and of backward
   float* zeros = nullptr;                                              // [4096] zero bias
+  float* drop_masks = nullptr;                                         // Swin: stochastic-depth masks of the step [B][kSwinBlocks][2]
   bool built = false, descs_dirty = true;
   std::vector<float> anchors;
   float* d_anchors = nullptr;
@@ -328,7 +330,6 @@ int op_conv(yb_train* t, TT* x, ConvRec* c, int relu, bool out_dense, const std:
         g.splits = splits < 1 ? 1 : splits;
         if (getenv("YOLACT_B200_TRAIN_NO_SPLITK")) g.splits = 1;              // tooling: A/B
       }
-      YB_REQUIRE(c->Cin == c->Cin_pad, YB_ERR_UNSUPPORTED, "train: conv %s Cin=%d is not a multiple of 64", c->wname.c_str(), c->Cin);
       TcPlan* gp = nullptr;
       YB_PROPAGATE(tc_plan_create_gemm(g, &gp));
       t->plans.push_back(gp);
@@ -455,12 +456,248 @@ int op_bn(yb_train* t, TT* y, const std::string& bn, int relu, TT* res, const st
   return YB_OK;
 }
 
+// ---- Swin-T ops (swin_train.cu kernels; the linear layers are op_conv with k = 1) ----
+// a linear layer of the reference (nn.Linear): a 1x1 conv record with the parameter's own names
+int swin_linear(yb_train* t, const std::string& prefix, int Cin, int Cout, bool bias, std::vector<ConvRec*>* all, ConvRec** out) {
+  ConvRec* c = new_conv(t, prefix, Cin, Cout, 1, 1, bias);
+  c->bias = t->zeros;
+  if (bias) { c->bias_idx = t->bidx.at(c->bname); c->bsum = stats_take(t, 2 * (size_t)(c->Cout_pad < 64 ? 64 : c->Cout_pad)); }
+  YB_PROPAGATE(alloc_conv(t, c, true));
+  all->push_back(c);
+  *out = c;
+  return YB_OK;
+}
+
+// copies a parameter gradient reduced in the statistics arena to the bound gradient buffer at the end of the backward pass
+void tail_copy(yb_train* t, float* arena_off, const std::string& name, int n) {
+  const int ib = t->bidx.at(name);
+  t->bwd_tail.push_back([=](cudaStream_t s) { return launch_scale_copy((float*)((char*)t->stats + (size_t)arena_off), t->bound[ib].grad, n, 1.f, s); });
+}
+
+// LayerNorm `prm` over the channels of x (per-token mean / rstd kept for the backward pass)
+int op_ln(yb_train* t, TT* x, const std::string& prm, const std::string& yname, TT** out) {
+  const int B = t->B, C = x->C, H = x->H, dt = t->dt;
+  t->cur_label = "ln " + yname;
+  t->add_bound(prm + ".weight", C, 0); t->add_bound(prm + ".bias", C, 0);
+  const int ig = t->bidx.at(prm + ".weight"), ib = t->bidx.at(prm + ".bias");
+  TT* y = new_tensor(t, yname, C, H);
+  YB_PROPAGATE(alloc_data(t, y));
+  const long long rows = x->rows;
+  float* st = nullptr;                                             // mean | rstd per token row
+  YB_PROPAGATE(dev_alloc(t, (void**)&st, (size_t)2 * rows * 4));
+  void* xd = x->data; void* yd = y->data;
+  FWD_PUSH([=](cudaStream_t s) { return launch_ln_fwd(xd, 0, yd, t->bound[ig].data, t->bound[ib].data, st, st + rows, dt, B, C, H, s); });
+  float* dgb = stats_take(t, 2 * (size_t)C);
+  tail_copy(t, dgb, prm + ".weight", C);
+  tail_copy(t, dgb + C, prm + ".bias", C);
+  t->bwd_builders.push_back([=]() -> int {
+    t->cur_label = "ln-bwd " + y->name;
+    YB_REQUIRE(y->grad && y->grad_set, YB_ERR_STATE, "train: LayerNorm output %s has no gradient", y->name.c_str());
+    YB_PROPAGATE(ensure_grad(t, x));
+    void* dy = y->grad; void* dx = x->grad; const int acc = x->grad_set ? 1 : 0;
+    BWD_PUSH([=](cudaStream_t s) {
+      return launch_ln_bwd(xd, 0, dy, t->bound[ig].data, st, st + rows, dx, acc, (float*)((char*)t->stats + (size_t)dgb), dt, B, C, H, s);
+    });
+    x->grad_set = true;
+    return YB_OK;
+  });
+  *out = y;
+  return YB_OK;
+}
+
+// x + m / keep * y with block `blk`'s mask of `branch` (0 attention, 1 MLP)
+int op_drop_residual(yb_train* t, TT* x, TT* y, int blk, int branch, const std::string& zname, TT** out) {
+  const int B = t->B, dt = t->dt;
+  t->cur_label = "residual " + zname;
+  YB_REQUIRE(x->C == y->C && x->H == y->H, YB_ERR_INVALID, "train: residual %s: shapes differ", zname.c_str());
+  TT* z = new_tensor(t, zname, x->C, x->H);
+  YB_PROPAGATE(alloc_data(t, z));
+  const long long per_img = (long long)(x->H + 2) * (x->H + 2) * x->C;
+  void* xd = x->data; void* yd = y->data; void* zd = z->data;
+  FWD_PUSH([=](cudaStream_t s) { return launch_drop_residual(xd, yd, zd, t->drop_masks, blk, branch, dt, B, per_img, s); });
+  t->bwd_builders.push_back([=]() -> int {
+    t->cur_label = "residual-bwd " + z->name;
+    YB_REQUIRE(z->grad && z->grad_set && !y->grad_set, YB_ERR_STATE, "train: residual %s: gradient state", z->name.c_str());
+    YB_PROPAGATE(ensure_grad(t, x)); YB_PROPAGATE(ensure_grad(t, y));
+    void* dz = z->grad; void* dx = x->grad; void* dy = y->grad; const int acc = x->grad_set ? 1 : 0;
+    BWD_PUSH([=](cudaStream_t s) { return launch_drop_residual_bwd(dz, dx, acc, dy, t->drop_masks, blk, branch, dt, B, per_img, s); });
+    x->grad_set = true; y->grad_set = true;
+    return YB_OK;
+  });
+  *out = z;
+  return YB_OK;
+}
+
+// (shifted-)window attention over the qkv linear's output (its only consumer)
+int op_attn(yb_train* t, TT* qkv, ConvRec* cq, const std::string& p, int heads, int shift, TT** out) {
+  const int B = t->B, dt = t->dt, C = qkv->C / 3, H = qkv->H;
+  t->cur_label = "attn " + p;
+  YB_REQUIRE(qkv->C == 3 * C && cq->Cout_pad == 3 * C, YB_ERR_INVALID, "train: attention %s: qkv width %d", p.c_str(), qkv->C);
+  const std::string tname = p + ".attn.relative_position_bias_table";
+  t->add_bound(tname, 169 * heads, 0);
+  const int iq = cq->bias_idx, it = t->bidx.at(tname);
+  TT* o = new_tensor(t, p + ".attn", C, H);
+  YB_PROPAGATE(alloc_data(t, o));
+  float* lse = nullptr;
+  YB_PROPAGATE(dev_alloc(t, (void**)&lse, (size_t)qkv->rows * heads * 4));
+  void* qd = qkv->data; void* od = o->data;
+  FWD_PUSH([=](cudaStream_t s) { return launch_wattn_fwd(qd, t->bound[iq].data, t->bound[it].data, od, lse, dt, B, H, C, heads, shift, s); });
+  float* dtab = stats_take(t, 169 * (size_t)heads);
+  tail_copy(t, dtab, tname, 169 * heads);
+  float* dbias = cq->bsum;                                         // the qkv bias sums: the padding tokens' dK / dV land there too
+  t->bwd_builders.push_back([=]() -> int {
+    t->cur_label = "attn-bwd " + o->name;
+    YB_REQUIRE(o->grad && o->grad_set && !qkv->grad_set, YB_ERR_STATE, "train: attention %s: gradient state", o->name.c_str());
+    YB_PROPAGATE(ensure_grad(t, qkv));
+    void* dout = o->grad; void* dq = qkv->grad;
+    BWD_PUSH([=](cudaStream_t s) {
+      return launch_wattn_bwd(qd, t->bound[iq].data, t->bound[it].data, dout, lse, dq, (float*)((char*)t->stats + (size_t)dtab),
+                              (float*)((char*)t->stats + (size_t)dbias), dt, B, H, C, heads, shift, s);
+    });
+    qkv->grad_set = true;
+    return YB_OK;
+  });
+  *out = o;
+  return YB_OK;
+}
+
+// exact-erf GELU of fc1's stored pre-activation (its only consumer)
+int op_gelu(yb_train* t, TT* h, const std::string& gname, TT** out) {
+  const int dt = t->dt;
+  t->cur_label = "gelu " + gname;
+  TT* g = new_tensor(t, gname, h->C, h->H);
+  YB_PROPAGATE(alloc_data(t, g));
+  const long long n = h->rows * h->C;
+  void* hd = h->data; void* gd = g->data;
+  FWD_PUSH([=](cudaStream_t s) { return launch_gelu_fwd(hd, gd, dt, n, s); });
+  t->bwd_builders.push_back([=]() -> int {
+    YB_REQUIRE(g->grad && g->grad_set && !h->grad_set, YB_ERR_STATE, "train: GELU %s: gradient state", g->name.c_str());
+    YB_PROPAGATE(ensure_grad(t, h));
+    void* dg = g->grad; void* dh = h->grad;
+    BWD_PUSH([=](cudaStream_t s) { return launch_gelu_bwd(hd, dg, dh, dt, n, s); });
+    h->grad_set = true;
+    return YB_OK;
+  });
+  *out = g;
+  return YB_OK;
+}
+
+// patch-merging gather [x0 | x1 | x2 | x3] (the LayerNorm and the reduction follow as op_ln / op_conv)
+int op_merge(yb_train* t, TT* x, const std::string& mname, TT** out) {
+  const int B = t->B, dt = t->dt, C = x->C, Hin = x->H, Hout = (Hin + 1) / 2;
+  t->cur_label = "merge " + mname;
+  TT* m = new_tensor(t, mname, 4 * C, Hout);
+  YB_PROPAGATE(alloc_data(t, m));
+  void* xd = x->data; void* md = m->data;
+  FWD_PUSH([=](cudaStream_t s) { return launch_merge_fwd(xd, md, dt, B, C, Hin, Hout, s); });
+  t->bwd_builders.push_back([=]() -> int {
+    YB_REQUIRE(m->grad && m->grad_set, YB_ERR_STATE, "train: patch merge %s has no gradient", m->name.c_str());
+    YB_PROPAGATE(ensure_grad(t, x));
+    void* dm = m->grad; void* dx = x->grad; const int acc = x->grad_set ? 1 : 0;
+    BWD_PUSH([=](cudaStream_t s) { return launch_merge_bwd(dm, dx, acc, dt, B, C, Hin, Hout, s); });
+    x->grad_set = true;
+    return YB_OK;
+  });
+  *out = m;
+  return YB_OK;
+}
+
+// Swin-T backbone (modules/swin_transformer.py:436-518, as net.cu's depth-0 program): patch embedding, 4 stages of (shifted-)window
+// blocks with stochastic depth, patch merging; couts[1..3] = backbone.norm1..3 (tensors "c3", "c4", "c5")
+int build_swin(yb_train* t, std::vector<ConvRec*>* all, TT** couts) {
+  const int B = t->B, S = t->S, dt = t->dt, Hg = (S + 3) / 4;
+  const int depths[4] = {2, 2, 6, 2}, heads[4] = {3, 6, 12, 24};
+  YB_PROPAGATE(dev_alloc(t, (void**)&t->drop_masks, (size_t)B * kSwinBlocks * 2 * 4));
+  {
+    float* masks = t->drop_masks;
+    t->cur_label = "drop-path masks";
+    FWD_PUSH([=](cudaStream_t s) { return launch_drop_path_masks(t->p_seed, masks, B, s); });
+  }
+  // ---- patch embedding: conv 4x4 / 4 (fp32 output) + LayerNorm; backward: LayerNorm, then the conv's weight and bias gradient ----
+  const std::string pe = "backbone.patch_embed";
+  t->add_bound(pe + ".proj.weight", 96 * 48, 0); t->add_bound(pe + ".proj.bias", 96, 0);
+  t->add_bound(pe + ".norm.weight", 96, 0); t->add_bound(pe + ".norm.bias", 96, 0);
+  TT* x = new_tensor(t, "patch_embed", 96, Hg);
+  YB_PROPAGATE(alloc_data(t, x));
+  {
+    t->cur_label = "patch embed";
+    const long long rows = x->rows;
+    float *raw = nullptr, *draw = nullptr, *st = nullptr;
+    YB_PROPAGATE(dev_alloc(t, (void**)&raw, (size_t)rows * 96 * 4));
+    YB_PROPAGATE(dev_alloc(t, (void**)&draw, (size_t)rows * 96 * 4));
+    YB_PROPAGATE(dev_alloc(t, (void**)&st, (size_t)2 * rows * 4));
+    const int iw = t->bidx.at(pe + ".proj.weight"), ib = t->bidx.at(pe + ".proj.bias"), ig = t->bidx.at(pe + ".norm.weight"),
+              ibe = t->bidx.at(pe + ".norm.bias");
+    float* img = t->d_img; void* xd = x->data;
+    FWD_PUSH([=](cudaStream_t s) { return launch_pe_conv(img, t->bound[iw].data, t->bound[ib].data, raw, B, S, Hg, s); });
+    FWD_PUSH([=](cudaStream_t s) { return launch_ln_fwd(raw, 1, xd, t->bound[ig].data, t->bound[ibe].data, st, st + rows, dt, B, 96, Hg, s); });
+    float* dgb = stats_take(t, 2 * 96);
+    float* dwb = stats_take(t, 96 * 48 + 96);
+    tail_copy(t, dgb, pe + ".norm.weight", 96); tail_copy(t, dgb + 96, pe + ".norm.bias", 96);
+    tail_copy(t, dwb, pe + ".proj.weight", 96 * 48); tail_copy(t, dwb + 96 * 48, pe + ".proj.bias", 96);
+    TT* xx = x;
+    t->bwd_builders.push_back([=]() -> int {
+      t->cur_label = "patch embed bwd";
+      YB_REQUIRE(xx->grad && xx->grad_set, YB_ERR_STATE, "train: patch embedding has no gradient");
+      void* dy = xx->grad;
+      BWD_PUSH([=](cudaStream_t s) {
+        return launch_ln_bwd(raw, 1, dy, t->bound[ig].data, st, st + rows, draw, 0, (float*)((char*)t->stats + (size_t)dgb), dt, B, 96, Hg, s);
+      });
+      BWD_PUSH([=](cudaStream_t s) {
+        float* w = (float*)((char*)t->stats + (size_t)dwb);
+        return launch_pe_wgrad(img, draw, w, w + 96 * 48, B, S, Hg, s);
+      });
+      return YB_OK;
+    });
+  }
+  // ---- stages ----
+  int blk = 0;
+  for (int st = 0; st < 4; ++st) {
+    const int C = 96 << st;
+    for (int b = 0; b < depths[st]; ++b, ++blk) {
+      const std::string p = "backbone.layers." + std::to_string(st) + ".blocks." + std::to_string(b);
+      TT *t1, *qkv, *att, *y, *x1, *t2, *h, *g, *y2;
+      ConvRec *cq, *cp, *c1, *c2;
+      YB_PROPAGATE(op_ln(t, x, p + ".norm1", p + ".norm1", &t1));
+      YB_PROPAGATE(swin_linear(t, p + ".attn.qkv", C, 3 * C, true, all, &cq));
+      YB_PROPAGATE(op_conv(t, t1, cq, 0, false, p + ".attn.qkv", &qkv));
+      YB_PROPAGATE(op_attn(t, qkv, cq, p, heads[st], (b % 2) ? 3 : 0, &att));
+      YB_PROPAGATE(swin_linear(t, p + ".attn.proj", C, C, true, all, &cp));
+      YB_PROPAGATE(op_conv(t, att, cp, 0, false, p + ".attn.proj", &y));
+      YB_PROPAGATE(op_drop_residual(t, x, y, blk, 0, p + ".x1", &x1));
+      YB_PROPAGATE(op_ln(t, x1, p + ".norm2", p + ".norm2", &t2));
+      YB_PROPAGATE(swin_linear(t, p + ".mlp.fc1", C, 4 * C, true, all, &c1));
+      YB_PROPAGATE(op_conv(t, t2, c1, 0, false, p + ".mlp.fc1", &h));
+      YB_PROPAGATE(op_gelu(t, h, p + ".mlp.gelu", &g));
+      YB_PROPAGATE(swin_linear(t, p + ".mlp.fc2", 4 * C, C, true, all, &c2));
+      YB_PROPAGATE(op_conv(t, g, c2, 0, false, p + ".mlp.fc2", &y2));
+      YB_PROPAGATE(op_drop_residual(t, x1, y2, blk, 1, p + ".out", &x));
+    }
+    if (st > 0) YB_PROPAGATE(op_ln(t, x, "backbone.norm" + std::to_string(st), "c" + std::to_string(st + 2), &couts[st]));
+    if (st < 3) {
+      const std::string p = "backbone.layers." + std::to_string(st) + ".downsample";
+      TT *mg, *mn;
+      ConvRec* cr;
+      YB_PROPAGATE(op_merge(t, x, p + ".merge", &mg));
+      YB_PROPAGATE(op_ln(t, mg, p + ".norm", p + ".norm", &mn));
+      YB_PROPAGATE(swin_linear(t, p + ".reduction", 4 * C, 2 * C, false, all, &cr));
+      YB_PROPAGATE(op_conv(t, mn, cr, 0, false, p + ".reduction", &x));
+    }
+  }
+  return YB_OK;
+}
+
 int build(yb_train* t) {
   const yb_net_config& cfg = t->cfg;
   const int B = t->B, S = cfg.img_size, dt = t->dt;
   t->S = S; t->H1 = (S - 1) / 2 + 1; t->H2 = (t->H1 - 1) / 2 + 1;
   YB_PROPAGATE(dev_alloc(t, (void**)&t->zeros, 4096 * 4));
   YB_PROPAGATE(dev_alloc(t, (void**)&t->d_img, (size_t)B * 3 * S * S * 4));
+  TT* couts[4] = {nullptr, nullptr, nullptr, nullptr};
+  std::vector<ConvRec*> all_convs;
+  if (cfg.depth == 0) {
+    YB_PROPAGATE(build_swin(t, &all_convs, couts));
+  } else {
 
   // ---------------- stem: space-to-depth image -> 4-tap K=64 conv -> BN -> ReLU -> max-pool ----------------
   const int H1 = t->H1, Wp1 = H1 + 2;
@@ -529,9 +766,7 @@ int build(yb_train* t) {
   // ---------------- bottleneck stages (modules/resnet.py:46-98) ----------------
   const int nblk50[4] = {3, 4, 6, 3}, nblk101[4] = {3, 4, 23, 3};
   const int* nblk = cfg.depth == 50 ? nblk50 : nblk101;
-  TT* couts[4] = {nullptr, nullptr, nullptr, nullptr};
   int inpl = 64;
-  std::vector<ConvRec*> all_convs;
   for (int st = 0; st < 4; ++st) {
     const int planes = 64 << st;
     for (int b = 0; b < nblk[st]; ++b) {
@@ -564,9 +799,10 @@ int build(yb_train* t) {
     couts[st] = x;
   }
   t->by_name["c2"] = couts[0]; t->by_name["c3"] = couts[1]; t->by_name["c4"] = couts[2]; t->by_name["c5"] = couts[3];
+  }
 
   // ---------------- FPN (modules/yolact.py:57-89) ----------------
-  const int fin[3] = {512, 1024, 2048};
+  const int fin[3] = {couts[1]->C, couts[2]->C, couts[3]->C};
   ConvRec *lat[3], *pred[3], *down[2];
   auto biased = [&](const std::string& prefix, int Cin, int Cout, int k, int stride, ConvRec** out) -> int {
     ConvRec* c = new_conv(t, prefix, Cin, Cout, k, stride, true);
@@ -773,7 +1009,8 @@ int resolve_descs(yb_train* t) {
 // ================================================================================================
 extern "C" int yb_train_create(const yb_net_config* cfg, int batch, int precision, yb_train** out) {
   YB_REQUIRE(cfg && out, YB_ERR_INVALID, "yb_train_create: NULL argument");
-  YB_REQUIRE(cfg->depth == 50 || cfg->depth == 101, YB_ERR_UNSUPPORTED, "yb_train_create: depth=%d (the training engine covers the ResNet backbones)", cfg->depth);
+  YB_REQUIRE(cfg->depth == 50 || cfg->depth == 101 || cfg->depth == 0, YB_ERR_UNSUPPORTED,
+             "yb_train_create: depth=%d (the training engine covers ResNet-50 / 101 and Swin-T, depth 0)", cfg->depth);
   YB_REQUIRE(batch >= 1 && batch <= 256, YB_ERR_INVALID, "yb_train_create: batch=%d", batch);
   YB_REQUIRE(precision == YB_PREC_BF16 || precision == YB_PREC_FP16, YB_ERR_UNSUPPORTED, "yb_train_create: precision=%d (bf16 or fp16 operands)", precision);
   YB_REQUIRE(cfg->coef_dim == 32 && cfg->num_ratios >= 1 && cfg->num_ratios <= 3 && cfg->num_classes >= 2 && cfg->num_classes <= 129, YB_ERR_UNSUPPORTED,
@@ -987,7 +1224,8 @@ extern "C" uint64_t yb_train_launches_per_step(const yb_train* t) { return t ? t
 extern "C" int yb_train_read(yb_train* t, const char* name, int grad, float* out, int64_t out_count, int* C, int* H, void* stream) {
   YB_REQUIRE(t && name, YB_ERR_INVALID, "yb_train_read: NULL argument");
   {  // the network outputs the losses consume (dense fp32): "out.cls" [B,A,C], "out.box" [B,A,4], "out.coef" [B,A,K], "out.proto"
-     // [B,P,P,K], "out.seg" [B,Hs,Hs,ld] -- C / H report the last two extents
+     // [B,P,P,K], "out.seg" [B,Hs,Hs,ld]; Swin-T: the step's stochastic-depth masks "out.drop_path" [B,12,2] -- C / H report the last
+     // two extents
     const std::string n(name);
     const float* src = nullptr; int64_t cnt = 0; int c = 0, h = 0;
     if (n == "out.cls") { src = t->cls; c = t->cfg.num_classes; h = t->A; cnt = (int64_t)t->B * t->A * c; }
@@ -995,6 +1233,7 @@ extern "C" int yb_train_read(yb_train* t, const char* name, int grad, float* out
     else if (n == "out.coef") { src = t->coef; c = t->cfg.coef_dim; h = t->A; cnt = (int64_t)t->B * t->A * c; }
     else if (n == "out.proto") { src = t->proto; c = t->cfg.coef_dim; h = t->P; cnt = (int64_t)t->B * t->P * t->P * c; }
     else if (n == "out.seg") { src = t->seg; c = t->ld_seg; h = t->Hs; cnt = (int64_t)t->B * t->Hs * t->Hs * c; }
+    else if (n == "out.drop_path" && t->drop_masks) { src = t->drop_masks; c = 2; h = kSwinBlocks; cnt = (int64_t)t->B * kSwinBlocks * 2; }
     if (src) {
       YB_REQUIRE(!grad, YB_ERR_UNSUPPORTED, "yb_train_read: '%s' has no readable gradient", name);
       if (C) *C = c;

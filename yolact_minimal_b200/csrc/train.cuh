@@ -52,6 +52,32 @@ int launch_head_grad(const float* dcls, const float* dbox, const float* dcoef, c
                      int anchor_offset, int A_total, int ldo, void* out, cudaStream_t s);
 int launch_scale_copy(const float* src, float* dst, int n, float scale, cudaStream_t s);
 
+// counter hash of the device-side random draws (mask subset in losses.cu, stochastic depth in swin_train.cu)
+__device__ __forceinline__ uint32_t hash32(uint32_t x) { x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16; return x; }
+
+// ---- Swin-T training (swin_train.cu): 16-bit haloed token grids, fp32 statistics; dgb / dtable / dw / db / dbias accumulate ----
+constexpr int kSwinBlocks = 12;                                    // blocks over the four stages (2 + 2 + 6 + 2)
+__host__ __device__ inline float swin_drop_rate(int blk) { return 0.2f * (float)blk / (float)(kSwinBlocks - 1); }   // linspace(0, 0.2, 12)
+int launch_ln_fwd(const void* x, int x_f32, void* y, const float* g, const float* be, float* mean, float* rstd, int dt, int B, int C, int H,
+                  cudaStream_t s);
+int launch_ln_bwd(const void* x, int x_f32, const void* dy, const float* g, const float* mean, const float* rstd, void* dx, int accumulate,
+                  float* dgb /*[2C]: dgamma | dbeta*/, int dt, int B, int C, int H, cudaStream_t s);
+int launch_pe_conv(const float* img, const float* w, const float* bias, float* out /*fp32 haloed [..][96]*/, int B, int S, int Hg, cudaStream_t s);
+int launch_pe_wgrad(const float* img, const float* dy, float* dw /*[96*48]*/, float* db /*[96]*/, int B, int S, int Hg, cudaStream_t s);
+int launch_wattn_fwd(const void* qkv, const float* qkv_bias, const float* table, void* out, float* lse /*[rows][nH]*/, int dt, int B, int H, int C,
+                     int nH, int shift, cudaStream_t s);
+int launch_wattn_bwd(const void* qkv, const float* qkv_bias, const float* table, const void* dout, const float* lse, void* dqkv, float* dtable,
+                     float* dbias /*[3C]*/, int dt, int B, int H, int C, int nH, int shift, cudaStream_t s);
+int launch_gelu_fwd(const void* h, void* y, int dt, long long n, cudaStream_t s);
+int launch_gelu_bwd(const void* h, const void* dy, void* dh, int dt, long long n, cudaStream_t s);
+int launch_merge_fwd(const void* in, void* out, int dt, int B, int C, int Hin, int Hout, cudaStream_t s);
+int launch_merge_bwd(const void* dout, void* dx, int accumulate, int dt, int B, int C, int Hin, int Hout, cudaStream_t s);
+int launch_drop_path_masks(const uint32_t* seed_dev, float* masks /*[B][kSwinBlocks][2]*/, int B, cudaStream_t s);
+int launch_drop_residual(const void* x, const void* y, void* out, const float* masks, int blk, int branch, int dt, int B, long long per_img,
+                         cudaStream_t s);
+int launch_drop_residual_bwd(const void* dout, void* dx, int accumulate, void* dy, const float* masks, int blk, int branch, int dt, int B,
+                             long long per_img, cudaStream_t s);
+
 
 // losses.cu: yb_losses with the seed in device memory; total_gt / max_gt_per_image only size grids and the workspace (graph replay)
 constexpr int kLossMaxGt = 256;

@@ -6,7 +6,8 @@ torch provides what it provides everywhere else in this package: device memory (
 -- the engine reads them and writes their gradients through bound device pointers), streams, and the autograd / DDP plumbing:
 the step is ONE autograd.Function whose inputs are the parameters, so `loss.backward()` hands each parameter its gradient
 and DistributedDataParallel's hooks (train.py:76) all-reduce them over NCCL exactly as they do for the reference.
-ResNet backbones; 16-bit tensor-core operands (bf16 by default: gradients need the exponent range), fp32 accumulation,
+ResNet and Swin-T backbones (Swin-T: LayerNorm, window attention, GELU, patch merging and stochastic depth in csrc/swin_train.cu,
+its linear layers on the same convolution kernels); 16-bit tensor-core operands (bf16 by default: gradients need the exponent range), fp32 accumulation,
 statistics, losses and parameter gradients.
 """
 import ctypes
@@ -24,8 +25,8 @@ class TrainEngine:
     """One native training program (fixed batch size) bound to a Yolact module's parameters and BN buffers."""
 
     def __init__(self, module, batch, precision='bf16'):
-        if module.depth not in (50, 101):
-            raise NotImplementedError('the native training engine covers the ResNet backbones (res50 / res101 configs)')
+        if module.depth not in (50, 101, 0):
+            raise NotImplementedError('the native training engine covers the res50 / res101 / swin_tiny configs')
         if precision not in PRECISIONS:
             raise ValueError(f'training precision must be one of {list(PRECISIONS)}, got {precision!r}')
         self.L = _lib.lib()
@@ -114,11 +115,12 @@ class TrainEngine:
 
     def read_output(self, name):
         """Debug / parity tap: a network output as the losses saw it -- 'cls' [B,A,C] raw logits, 'box' [B,A,4], 'coef' [B,A,K] (tanh),
-        'proto' [B,P,P,K], 'seg' [B,Hs,Hs,C-1] (NHWC)."""
+        'proto' [B,P,P,K], 'seg' [B,Hs,Hs,C-1] (NHWC); Swin-T: 'drop_path' [B,12,2], the last step's stochastic-depth masks (block,
+        attention | MLP branch)."""
         C, H = ctypes.c_int(), ctypes.c_int()
         key = ('out.' + name).encode()
         _lib.check(self.L.yb_train_read(self.h, key, 0, None, 0, ctypes.byref(C), ctypes.byref(H), None), 'yb_train_read')
-        shape = (self.batch, H.value, C.value) if name in ('cls', 'box', 'coef') else (self.batch, H.value, H.value, C.value)
+        shape = (self.batch, H.value, C.value) if name in ('cls', 'box', 'coef', 'drop_path') else (self.batch, H.value, H.value, C.value)
         out = torch.empty(shape, dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             _lib.check(self.L.yb_train_read(self.h, key, 0, out.data_ptr(), out.numel(), ctypes.byref(C), ctypes.byref(H),
