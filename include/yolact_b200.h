@@ -277,6 +277,33 @@ YB_API int yb_draw_cutout(const uint8_t* img_bgr, int h, int w, const void* mask
                           int num_colors, const int32_t* crop_yyxx, const int64_t* crop_off, uint8_t* out_total,
                           uint8_t* out_crops, void* stream);
 
+/* Batched overlay: yb_draw_masks for B images of any sizes in one launch, with no host sync on the detection counts.
+ *   src / items: the raw images back to back and their HOST yb_val_aug_item table (the buffer yb_val_aug_batch reads); out
+ *   (src_bytes bytes, same layout) must not overlap src.  masks: bit-packed, image b's [max_det, h_b, ceil(w_b/32)] words from
+ *   masks + mask_off[b] (HOST int64 [B+1]; they must end at or before mask_off[b+1], and mask_off[B] <= mask_words):
+ *   yb_mask_assemble_batch's buffer.  ids int32 [B, max_det]; count int32 [B] (DEVICE).
+ *   Image b blends its first min(count[b], max_det) masks exactly as yb_draw_masks does; an image with count[b] <= 0 is copied
+ *   unchanged (draw_img returns img_origin when nothing is left).
+ * Every size and offset is checked on the host before the launch (YB_ERR_INVALID); the geometry table then goes through the
+ * page-locked staging of yb_mask_assemble_batch, so the call queues without waiting for the stream.
+ * workspace: yb_draw_masks_batch_workspace_bytes(B). */
+YB_API size_t yb_draw_masks_batch_workspace_bytes(int batch);
+YB_API int yb_draw_masks_batch(const uint8_t* src, int64_t src_bytes, const yb_val_aug_item* items, int batch, const uint32_t* masks,
+                               const int64_t* mask_off, int64_t mask_words, int max_det, const int32_t* ids, const int32_t* count,
+                               const uint8_t* palette, int num_colors, void* workspace, size_t workspace_bytes, uint8_t* out,
+                               void* stream);
+
+/* cfg.save_lincomb: utils/output_utils.py:276-305 draw_lincomb for detection 0 of each of B images, one launch.
+ *   proto float32 [B,P,P,K], coef float32 [B,max_det,K], count int32 [B] (DEVICE; NULL = every image): an image with
+ *   count <= 0 is not written.  lut uint8 [256,3] (cv2.COLORMAP_WINTER); out uint8 [B, 4P, 8P, 3].  K must be 32
+ *   (the 4 x 8 grid; anything else is YB_ERR_UNSUPPORTED).
+ *   Cell (r, c) shows channel ch = order[8r + c], order = the 32 coefficients by |coef| descending, ties to the lower channel
+ *   (NaN last): x = fp32(fp32(proto[y,x,ch] / max_ch) * coef[ch]) with max_ch the channel's maximum over its P x P plane (NaN if
+ *   it holds one), u = ((double)x + 1) * 127.5, byte = low byte of the int32 truncation of u (x86-64's cast: NaN and values
+ *   outside int32 give 0), pixel = lut[byte].  The reference's tie order is numpy's unstable argsort; this one is stable. */
+YB_API int yb_draw_lincomb(const float* proto, const float* coef, const int32_t* count, int batch, int max_det, int proto_size,
+                           int coef_dim, const uint8_t* lut, uint8_t* out, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Network: ResNet-50/101 + FPN + ProtoNet + prediction heads (modules/resnet.py,
  * modules/yolact.py:12-164), eval forward.  Weights are handed over by their reference

@@ -105,6 +105,10 @@ PROTOTYPES = {
     'yb_mask_rle': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp]),
     'yb_draw_masks': (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, vp, C.c_int, vp, vp]),
     'yb_draw_cutout': (C.c_int, [vp, C.c_int, C.c_int, vp, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]),
+    'yb_draw_masks_batch_workspace_bytes': (C.c_size_t, [C.c_int]),
+    'yb_draw_masks_batch': (C.c_int, [vp, C.c_int64, vp, C.c_int, vp, vp, C.c_int64, C.c_int, vp, vp, vp, C.c_int, vp, C.c_size_t,
+                                      vp, vp]),
+    'yb_draw_lincomb': (C.c_int, [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]),
     'yb_eval_state_bytes': (C.c_size_t, [C.POINTER(EvalParams)]),
     'yb_eval_match_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.POINTER(EvalParams)]),
     'yb_eval_ap_workspace_bytes': (C.c_size_t, [C.c_int64, C.POINTER(EvalParams)]),

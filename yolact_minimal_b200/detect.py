@@ -1,0 +1,221 @@
+"""Detection in batches on the GPU: the reference's detect.py with the same arguments and outputs (results/images/{name},
+lincomb_{name}, the cutout images, results/videos/{name}), fed `--det_bs` images or video frames at a time:
+
+    one H2D copy -> val_aug_batch -> net(images) -> detect_batched -> visible_count -> after_nms_batched
+      -> blend_masks_batched (unless hide_mask) -> lincomb_batched (save_lincomb) -> async D2H copies        (per batch, no host sync)
+    draw_labels (cv2 boxes, labels, fps) -> cv2.imwrite / VideoWriter.write                                  (host, one batch behind)
+
+The host waits for batch i only after batch i+1 is queued, so the cv2 pass of one batch runs under the device work of the next.
+Every written image equals the reference's per-image loop (val_aug, net, nms, after_nms, draw_img) on this package bit for bit:
+the forward is batch-invariant at a fixed max_batch, detect_batched treats images independently, visual_thre keeps a prefix of
+each image's score-sorted detections, after_nms_batched equals after_nms per image and bit-packed masks draw as float masks do.
+
+    python -m yolact_minimal_b200.detect --weight weights/best_30.5_res101_coco_392000.pth --image images --det_bs 16
+"""
+import argparse
+import re
+import time
+
+import torch
+
+from .utils.augmentations import val_aug_batch
+from .utils.coco import DetectImages, PackedDetectBatch, detect_collate
+from .utils.common_utils import ProgressBar
+from .utils.output_utils import (after_nms_batched, blend_masks_batched, cutout_masks, detect_batched, draw_labels, lincomb_batched,
+                                 visible_count)
+
+
+class _HostBuffers:
+    """Page-locked buffers the D2H copies of one batch land in; detect keeps two and alternates, so a batch's results stay put
+    while the next batch's copies are queued."""
+
+    def __init__(self):
+        self._bufs = {}
+
+    def take(self, key, t):
+        buf = self._bufs.get(key)
+        if buf is None or buf.numel() < t.numel() or buf.dtype != t.dtype:
+            buf = self._bufs[key] = torch.empty(t.numel(), dtype=t.dtype, pin_memory=True)
+        buf = buf[:t.numel()]
+        buf.copy_(t.reshape(-1), non_blocking=True)
+        return buf.view(t.shape)
+
+
+class _Pending:
+    """A queued batch: what its host pass needs once `done` has completed."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
+def enqueue(net, cfg, packed, host):
+    """Queues one batch's device work and the copies of its results into `host` (a _HostBuffers); never waits for the device."""
+    dev = next(net.parameters()).device
+    src = packed.buffer.to(dev, non_blocking=packed.buffer.is_pinned())
+    with torch.no_grad():
+        images = val_aug_batch(src, packed.items, cfg.img_size, dev)
+        class_p, box_p, coef_p, proto_p = net(images)
+    det = detect_batched(class_p, box_p, coef_p, net.anchors, cfg)
+    det = dict(det, count=visible_count(det, cfg.visual_thre))
+    boxes_px, masks = after_nms_batched(det, proto_p, packed.sizes, crop=not cfg.no_crop)
+    out = {'count': det['count'], 'cls': det['cls'], 'score': det['score'], 'boxes': boxes_px}
+    if not cfg.hide_mask:
+        out['frames'] = blend_masks_batched(src, packed.items, det, masks, cfg.num_classes)
+    if cfg.save_lincomb:
+        out['lincomb'] = lincomb_batched(proto_p, det)
+    res = {k: host.take(k, v) for k, v in out.items()}
+    done = torch.cuda.Event()
+    done.record()
+    return _Pending(packed=packed, src=src, det=det, masks=masks, res=res, done=done)
+
+
+def finish(p, cfg, emit, fps=None):
+    """Waits for a queued batch and runs the host pass of draw_img on each image: lincomb_{name} (save_lincomb), the cutout images,
+    then the boxes / labels / fps; emit(name, image) receives each drawn image."""
+    import cv2
+    p.done.synchronize()
+    r, packed = p.res, p.packed
+    count = r['count'].numpy()
+    for b, (h, w) in enumerate(packed.sizes):
+        n, name = int(count[b]), packed.names[b]
+        if n <= 0:                                        # after_nms returned None: draw_img gives back img_origin
+            emit(name, packed.image(b))
+            continue
+        if cfg.save_lincomb:
+            cv2.imwrite(f'results/images/lincomb_{name}', r['lincomb'][b].numpy())
+        ids_np, scores_np, boxes_np = r['cls'][b, :n].numpy(), r['score'][b, :n].numpy(), r['boxes'][b, :n].numpy()
+        if cfg.hide_mask:
+            img = packed.image(b)                         # drawn in place, as the reference draws into img_origin
+        else:
+            off = int(packed.items[b]['img_off'])
+            if cfg.cutout:
+                src_b = p.src[off:off + h * w * 3].view(h, w, 3)
+                total, crops = cutout_masks(src_b, p.det['cls'][b, :n], boxes_np, p.masks[b][:n], cfg.num_classes)
+                cv2.imwrite(f'results/images/{name}_total_obj.jpg', total)
+                for i, crop in enumerate(crops):
+                    cv2.imwrite(f'results/images/{name}_{i}.jpg', crop)
+            img = r['frames'][off:off + h * w * 3].numpy().reshape(h, w, 3)
+        emit(name, draw_labels(img, ids_np, scores_np, boxes_np, cfg, fps))
+
+
+def run(net, cfg, batches, emit, progress=None):
+    """Detects every batch of `batches` (PackedDetectBatch) with one batch in flight while the host draws the previous one.
+    progress(done_images, images_per_second) is called after each batch; the rate is also the fps the real_time view shows."""
+    hosts = (_HostBuffers(), _HostBuffers())
+    pending, done, start, fps = None, 0, time.perf_counter(), 0.0
+    for i, packed in enumerate(batches):
+        cur = enqueue(net, cfg, packed, hosts[i % 2])
+        if pending is not None:
+            finish(pending, cfg, emit, fps)
+            done += len(pending.packed)
+            fps = done / (time.perf_counter() - start)
+            if progress:
+                progress(done, fps)
+        pending = cur
+    if pending is not None:
+        finish(pending, cfg, emit, fps)
+        done += len(pending.packed)
+        if progress:
+            progress(done, done / (time.perf_counter() - start))
+
+
+def detect_images(net, cfg, det_bs, num_workers=2):
+    """The reference's image loop (detect.py:52-99): every cfg.image/*.jpg, drawn to results/images/{name}."""
+    import cv2
+    from torch.utils.data import DataLoader
+    dataset = DetectImages(cfg)
+    assert len(dataset) > 0, 'No .jpg images found.'
+    loader = DataLoader(dataset, det_bs, num_workers=num_workers, shuffle=False, pin_memory=True, collate_fn=detect_collate)
+    bar = ProgressBar(40, len(dataset))
+
+    def progress(done, fps):
+        print(f'\rTesting: {bar.get_bar(done)} {done}/{len(dataset)}, total fps: {fps:.2f}', end='')
+
+    run(net, cfg, loader, lambda name, img: cv2.imwrite(f'results/images/{name}', img), progress)
+    print('\nFinished, saved in: results/images.')
+
+
+def _video_batches(vid, num_frames, det_bs):
+    frames = []
+    for _ in range(num_frames):
+        ok, frame = vid.read()
+        if not ok:
+            break
+        frames.append(frame)
+        if len(frames) == det_bs:
+            yield PackedDetectBatch(frames, [None] * len(frames)).pin_memory()     # the reference names no frame
+            frames = []
+    if frames:
+        yield PackedDetectBatch(frames, [None] * len(frames)).pin_memory()
+
+
+def detect_video(net, cfg, det_bs):
+    """The reference's video loop (detect.py:101-167): frames to results/videos/{name} (mp4v), or to a window with real_time."""
+    import cv2
+    vid = cv2.VideoCapture(cfg.video)
+    target_fps = round(vid.get(cv2.CAP_PROP_FPS))
+    frame_width = round(vid.get(cv2.CAP_PROP_FRAME_WIDTH))
+    frame_height = round(vid.get(cv2.CAP_PROP_FRAME_HEIGHT))
+    num_frames = round(vid.get(cv2.CAP_PROP_FRAME_COUNT))
+    name = cfg.video.split('/')[-1]
+    video_writer = cv2.VideoWriter(f'results/videos/{name}', cv2.VideoWriter_fourcc(*"mp4v"), target_fps, (frame_width, frame_height))
+    bar = ProgressBar(40, max(num_frames, 1))
+
+    def emit(_, frame):
+        if cfg.real_time:
+            cv2.imshow('Detection', frame)
+            cv2.waitKey(1)
+        else:
+            video_writer.write(frame)
+
+    def progress(done, fps):
+        print(f'\rDetecting: {bar.get_bar(done)} {done}/{num_frames}, total fps: {fps:.2f}', end='')
+
+    run(net, cfg, _video_batches(vid, num_frames, det_bs), emit, progress)
+    if not cfg.real_time:
+        print(f'\n\nFinished, saved in: results/videos/{name}')
+    vid.release()
+    video_writer.release()
+
+
+def main(argv=None):
+    from .config import get_config
+    from .modules.yolact import Yolact
+    parser = argparse.ArgumentParser(description='YOLACT Detection.')
+    parser.add_argument('--weight', default='weights/best_30.5_res101_coco_392000.pth', type=str)
+    parser.add_argument('--image', default=None, type=str, help='The folder of images for detecting.')
+    parser.add_argument('--video', default=None, type=str, help='The path of the video to evaluate.')
+    parser.add_argument('--img_size', type=int, default=544, help='The image size for validation.')
+    parser.add_argument('--traditional_nms', default=False, action='store_true', help='Whether to use traditional nms.')
+    parser.add_argument('--hide_mask', default=False, action='store_true', help='Hide masks in results.')
+    parser.add_argument('--hide_bbox', default=False, action='store_true', help='Hide boxes in results.')
+    parser.add_argument('--hide_score', default=False, action='store_true', help='Hide scores in results.')
+    parser.add_argument('--cutout', default=False, action='store_true', help='Cut out each object and save.')
+    parser.add_argument('--save_lincomb', default=False, action='store_true', help='Show the generating process of masks.')
+    parser.add_argument('--no_crop', default=False, action='store_true',
+                        help='Do not crop the output masks with the predicted bounding box.')
+    parser.add_argument('--real_time', default=False, action='store_true', help='Show the detection results real-timely.')
+    parser.add_argument('--visual_thre', default=0.3, type=float,
+                        help='Detections with a score under this threshold will be removed.')
+    parser.add_argument('--det_bs', default=1, type=int, help='Images (or video frames) per batch on the GPU.')
+    args = parser.parse_args(argv)
+    if args.det_bs < 1:
+        parser.error(f'--det_bs must be >= 1, got {args.det_bs}')
+    prefix = re.findall(r'best_\d+\.\d+_', args.weight)[0]
+    suffix = re.findall(r'_\d+\.pth', args.weight)[0]
+    args.cfg = args.weight.split(prefix)[-1].split(suffix)[0]
+    cfg = get_config(args, mode='detect')
+    cfg.max_batch = args.det_bs                      # the forward is batch-invariant at a fixed max_batch
+
+    net = Yolact(cfg)
+    net.load_weights(cfg.weight, cfg.cuda)
+    net.eval()
+    net = net.cuda()
+    if cfg.image is not None:
+        detect_images(net, cfg, args.det_bs)
+    elif cfg.video is not None:
+        detect_video(net, cfg, args.det_bs)
+
+
+if __name__ == '__main__':
+    main()

@@ -9,12 +9,16 @@ train_aug_batch) augments it on the device.
 'val' (COCOValDetection, val_collate :31-35): each worker returns the raw uint8 image, the gts and the gt masks
 bit-packed on the host; val_collate packs a batch into a PackedValBatch, and yolact_minimal_b200.eval.evaluate runs
 val_aug on the device for the whole batch (utils.augmentations.val_aug_batch).
+
+'detect' (DetectImages, detect_collate :38-40): each worker reads one image of the folder; detect_collate packs a batch into a
+PackedDetectBatch, and yolact_minimal_b200.detect runs val_aug, the network and the drawing on the device for the whole batch.
 """
+import glob
 import os.path as osp
 
 import numpy as np
 
-from .augmentations import PackedTrainBatch, PackedValBatch, train_aug_plan
+from .augmentations import PackedTrainBatch, PackedValBatch, pack_images, train_aug_plan
 from .mask_utils import pack_masks_host
 
 
@@ -129,3 +133,51 @@ class COCOValDetection:
         boxes = boxes / np.array([width, height, width, height])
         gt = np.hstack((boxes, np.expand_dims(labels, axis=1))).astype(np.float32)
         return np.ascontiguousarray(img), gt, pack_masks_host(masks), (height, width), img_id
+
+
+class PackedDetectBatch:
+    """A batch of images for yolact_minimal_b200.detect: `buffer` / `items` the raw uint8 BGR images back to back and their
+    yb_val_aug_item table (pack_images), `names` their file names, `sizes` their (h, w).  With DataLoader(pin_memory=True) the
+    loader's pin thread page-locks the buffer."""
+
+    def __init__(self, images, names):
+        self.buffer, self.items = pack_images(images)
+        self.names = list(names)
+        self.sizes = [(int(h), int(w)) for _, h, w in self.items.tolist()]
+
+    def __len__(self):
+        return len(self.items)
+
+    def pin_memory(self):
+        self.buffer = self.buffer.pin_memory()
+        return self
+
+    def image(self, b):
+        """Image b as a numpy view [h,w,3] of the (host) buffer."""
+        off, h, w = self.items[b].tolist()
+        return self.buffer.numpy()[off:off + h * w * 3].reshape(h, w, 3)
+
+
+def detect_collate(batch):
+    """Packs a batch of DetectImages samples."""
+    return PackedDetectBatch([s[0] for s in batch], [s[1] for s in batch])
+
+
+class DetectImages:
+    """The reference's COCODetection(cfg, mode='detect') images (utils/coco.py:56-67): the sorted glob(cfg.image + '/*.jpg').
+    Returns (img_u8 [h,w,3] BGR, file name); val_aug runs on the device for a whole batch."""
+
+    def __init__(self, cfg):
+        self.image_path = glob.glob(cfg.image + '/*.jpg')
+        self.image_path.sort()
+
+    def __len__(self):
+        return len(self.image_path)
+
+    def __getitem__(self, index):
+        import cv2
+        img_name = self.image_path[index]
+        img = cv2.imread(img_name)
+        if img is None:
+            raise RuntimeError(f'cannot read image {img_name}')
+        return np.ascontiguousarray(img), img_name.split(osp.sep)[-1]

@@ -3,7 +3,8 @@
 yb_detect / yb_mask_assemble / yb_draw_masks (include/yolact_b200.h).  Same arguments, same return
 tuples, same "(None, ...)" convention for "no detections".  `detect_batched` and `after_nms_batched`
 are the batched forms the reference lacks (its nms() squeezes a batch of 1, output_utils.py:127-130);
-`blend_masks` is draw_img's overlay on device-resident frames.
+`blend_masks` is draw_img's overlay on device-resident frames, `blend_masks_batched` the same for a batch of images of any sizes,
+and `lincomb_batched` draw_lincomb (cfg.save_lincomb) for a batch.
 
 All inputs must be CUDA tensors (draw_img also takes numpy arrays, which it uploads); nothing here
 falls back to the CPU.
@@ -139,11 +140,13 @@ def after_nms(ids_p, class_p, box_p, coef_p, proto_p, img_h, img_w, cfg=None, im
         if not bool(keep.any()):
             return None, None, None, None
         ids_p, class_p, box_p, coef_p = ids_p[keep], class_p[keep], box_p[keep], coef_p[keep]
-    if cfg is not None and getattr(cfg, 'save_lincomb', False):
-        raise NotImplementedError('save_lincomb is a visualisation option (draw_lincomb); out of scope')
     dev = proto_p.device
     proto = proto_p.detach().to(torch.float32).contiguous()
     coef = coef_p.detach().to(torch.float32).contiguous()
+    if cfg is not None and getattr(cfg, 'save_lincomb', False):                   # :214-215
+        import cv2
+        lincomb = lincomb_batched(proto[None], {'coef': coef[None]})
+        cv2.imwrite(f'results/images/lincomb_{img_name}', lincomb[0].cpu().numpy())
     box = box_p.detach().to(torch.float32).contiguous()
     d, K = coef.shape
     P = proto.shape[0]
@@ -322,6 +325,87 @@ def blend_masks(img, ids, masks, num_classes):
     return out
 
 
+def visible_count(det, visual_thre):
+    """after_nms' visual_thre filter (utils/output_utils.py:204-212) for a detect_batched record, on the device and without a sync:
+    the record is sorted by descending score, so `score >= visual_thre` keeps a prefix of each image's detections; returns its
+    length per image (int32 [B]).  The comparison is after_nms' own (a float32 tensor against the Python float)."""
+    count = det['count']
+    if not visual_thre > 0:
+        return count
+    D = det['score'].shape[1]
+    live = torch.arange(D, device=count.device)[None] < count[:, None].long()
+    return (live & (det['score'] >= visual_thre)).sum(1, dtype=torch.int32)
+
+
+def blend_masks_batched(src, items, det, masks, num_classes):
+    """blend_masks for a batch of images of any sizes, in one yb_draw_masks_batch launch and without a host sync on the counts.
+    src: CUDA uint8 buffer holding the BGR images back to back, `items` its numpy yb_val_aug_item table (pack_images); det: a
+    record with 'count' [B] (DEVICE) and 'cls' [B,D]; masks: after_nms_batched's list of packed-mask views [D,h_b,ceil(w_b/32)].
+    Returns a new CUDA buffer laid out as src: image b blended with its first count[b] masks, or unchanged when count[b] <= 0."""
+    import numpy as np
+    from .augmentations import VAL_ITEM_DTYPE
+    count, cls = det['count'], det['cls']
+    _require_cuda(src, count, cls, *masks)
+    items = np.ascontiguousarray(items, dtype=VAL_ITEM_DTYPE)
+    B, D = int(cls.shape[0]), int(cls.shape[1])
+    if src.dtype != torch.uint8 or src.dim() != 1 or len(items) != B or len(masks) != B or tuple(count.shape) != (B,):
+        raise ValueError(f'src {src.dtype} {tuple(src.shape)}, {len(items)} items, {len(masks)} mask views and count '
+                         f'{tuple(count.shape)} do not describe {B} images')
+    storage = masks[0].untyped_storage()
+    for b, (m, (_, h, w)) in enumerate(zip(masks, items.tolist())):
+        if m.dtype != torch.int32 or tuple(m.shape) != (D, h, (w + 31) // 32) or not m.is_contiguous() or \
+                m.untyped_storage().data_ptr() != storage.data_ptr():
+            raise ValueError(f'mask view {b}: {m.dtype} {tuple(m.shape)} is not a contiguous [{D},{h},{(w + 31) // 32}] int32 view of '
+                             'the batch buffer')
+    base = storage.data_ptr()
+    off = np.asarray([m.storage_offset() for m in masks] + [masks[-1].storage_offset() + masks[-1].numel()], np.int64)
+    pal, nc = _palette(num_classes, src.device)
+    ids32, count32 = cls.to(torch.int32).contiguous(), count.to(torch.int32).contiguous()
+    out = torch.empty_like(src)
+    L = _lib.lib()
+    with torch.cuda.device(src.device):
+        ws = torch.empty(int(L.yb_draw_masks_batch_workspace_bytes(B)), dtype=torch.uint8, device=src.device)
+        _lib.check(L.yb_draw_masks_batch(src.data_ptr(), src.numel(), items.ctypes.data, B, base, off.ctypes.data, storage.nbytes() // 4,
+                                         D, ids32.data_ptr(), count32.data_ptr(), pal.data_ptr(), nc, ws.data_ptr(), ws.numel(),
+                                         out.data_ptr(), torch.cuda.current_stream().cuda_stream), 'yb_draw_masks_batch')
+    return out
+
+
+def _winter_lut(device):
+    key = ('winter', device.index)
+    lut = _palette_cache.get(key)
+    if lut is None:
+        import cv2
+        import numpy as np
+        # for uint8 input applyColorMap is this table lookup
+        table = cv2.applyColorMap(np.arange(256, dtype=np.uint8)[:, None], cv2.COLORMAP_WINTER)[:, 0]
+        lut = _palette_cache[key] = torch.from_numpy(np.ascontiguousarray(table)).to(device)
+    return lut
+
+
+def lincomb_batched(proto, det):
+    """draw_lincomb (utils/output_utils.py:276-305, cfg.save_lincomb) for detection 0 of each image, one yb_draw_lincomb launch.
+    proto [B,P,P,32] (Yolact.forward's proto); det: a record with 'coef' [B,D,32] and optionally 'count' [B] (DEVICE): images
+    with count <= 0 are left unwritten (zero).  Returns CUDA uint8 [B, 4P, 8P, 3], the BGR image cv2.imwrite writes.  Coefficients
+    of equal magnitude are ordered lower channel first (the reference's order for them is numpy's unstable argsort)."""
+    coef = det['coef']
+    count = det.get('count')
+    _require_cuda(proto, coef, *([] if count is None else [count]))
+    proto = proto.detach().to(torch.float32).contiguous()
+    coef = coef.detach().to(torch.float32).contiguous()
+    B, P, _, K = proto.shape
+    if tuple(proto.shape) != (B, P, P, K) or coef.dim() != 3 or coef.shape[0] != B or coef.shape[2] != K:
+        raise ValueError(f'proto {tuple(proto.shape)} does not match coef {tuple(coef.shape)}')
+    count32 = None if count is None else count.to(torch.int32).contiguous()
+    out = torch.zeros(B, 4 * P, 8 * P, 3, dtype=torch.uint8, device=proto.device)
+    L = _lib.lib()
+    with torch.cuda.device(proto.device):
+        _lib.check(L.yb_draw_lincomb(proto.data_ptr(), coef.data_ptr(), None if count32 is None else count32.data_ptr(), B,
+                                     int(coef.shape[1]), P, K, _winter_lut(proto.device).data_ptr(), out.data_ptr(),
+                                     torch.cuda.current_stream().cuda_stream), 'yb_draw_lincomb')
+    return out
+
+
 def cutout_masks(img, ids, boxes, masks, num_classes):
     """draw_img's cfg.cutout images (utils/output_utils.py:328-341) on the device.  Returns (total_obj [h,w,3], [crop_i]) as host
     uint8 arrays: total_obj = img where the semantic index is non-zero, else 255; crop_i = (img where masks_i, else 255)[y1:y2,
@@ -362,7 +446,6 @@ def draw_img(ids_p, class_p, box_p, mask_p, img_origin, cfg, img_name=None, fps=
         return img_origin
     import cv2
     import numpy as np
-    from ..config import COLORS
     args = (ids_p, class_p, box_p, mask_p)
     if any(isinstance(t, torch.Tensor) and not t.is_cuda for t in args):
         raise _lib.YolactB200Error('draw_img needs CUDA tensors or numpy arrays (no CPU fallback)')
@@ -384,6 +467,15 @@ def draw_img(ids_p, class_p, box_p, mask_p, img_origin, cfg, img_name=None, fps=
             for i, crop in enumerate(crops):
                 cv2.imwrite(f'results/images/{img_name}_{i}.jpg', crop)
         img_fused = fused_d.cpu().numpy()
+    return draw_labels(img_fused, ids_np, scores_np, boxes_np, cfg, fps)
+
+
+def draw_labels(img_fused, ids_np, scores_np, boxes_np, cfg, fps=None):
+    """draw_img's host pass (utils/output_utils.py:343-369) on the overlaid uint8 image: boxes and labels (drawn in place) unless
+    cfg.hide_bbox, and with cfg.real_time the fps text on a darkened corner (a new array).  Returns the image."""
+    import cv2
+    import numpy as np
+    from ..config import COLORS
     scale = 0.6
     thickness = 1
     font = cv2.FONT_HERSHEY_DUPLEX
