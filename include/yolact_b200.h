@@ -517,6 +517,36 @@ YB_API int yb_train_backward(yb_train* t, const float* loss_grad, void* stream);
 YB_API int yb_train_read(yb_train* t, const char* name, int grad, float* out, int64_t out_count, int* C, int* H, void* stream);
 YB_API uint64_t yb_train_launches_per_step(const yb_train* t);
 
+/* ------------------------------------------------------------------------------------------
+ * Optimizer step: torch's foreach SGD (momentum, L2 weight decay, dampening 0) and AdamW (decoupled weight decay) on CUDA,
+ * bit for bit, over every parameter in one launch.  The parameters stay where the caller keeps them (params_device[i],
+ * counts[i] fp32 elements); their gradient is ONE flat fp32 buffer, the parameters concatenated in the order given here (the
+ * order of a yb_train program's kind-0 tensors, so yb_train_bind's gradient buffer can be passed as is).  The optimizer owns
+ * its state (SGD: momentum buffer; AdamW: exp_avg, exp_avg_sq; zero at creation) and does not belong to a yb_train: several
+ * programs (batch sizes) bound to the same parameters step the same state.
+ *   create -> [step]* -> destroy
+ * yb_optim_step: p <- update(p, grad_scale * grad_flat) with learning rate `lr`; the per-step scalars (bias corrections) are
+ * computed on the host in double from the call count, as torch computes them.  Asynchronous on `stream`; touches nothing
+ * outside the listed parameter ranges.  Must run on the device the optimizer was created on.
+ * ---------------------------------------------------------------------------------------- */
+typedef struct yb_optim yb_optim;
+typedef enum { YB_OPTIM_SGD = 0, YB_OPTIM_ADAMW = 1 } yb_optim_kind;
+typedef struct {
+  int kind;                              /* yb_optim_kind */
+  double momentum, dampening;            /* SGD: momentum > 0, dampening 0 */
+  double weight_decay;                   /* SGD: added to the gradient; AdamW: decoupled (p *= 1 - lr * weight_decay) */
+  double beta1, beta2, eps;              /* AdamW: 0.5 < beta1 < 1, 0 <= beta2 < 1 */
+} yb_optim_params;
+
+YB_API int yb_optim_create(const yb_optim_params* p, int n, float* const* params_device, const int64_t* counts, yb_optim** out);
+YB_API int yb_optim_step(yb_optim* o, const float* grad_flat, double lr, float grad_scale, void* stream);
+/* debug / parity tap: state `which` (0: SGD momentum buffer | AdamW exp_avg, 1: AdamW exp_avg_sq) in the gradient's layout,
+ * out_count = yb_optim_num_elements (device; asynchronous on `stream`) */
+YB_API int yb_optim_read_state(const yb_optim* o, int which, float* out, int64_t out_count, void* stream);
+/* elements of the flat gradient (sum of counts) */
+YB_API int64_t yb_optim_num_elements(const yb_optim* o);
+YB_API void yb_optim_destroy(yb_optim* o);
+
 #ifdef __cplusplus
 }
 #endif

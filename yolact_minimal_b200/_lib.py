@@ -50,6 +50,11 @@ class TrainHparams(C.Structure):
                 ('bn_momentum', C.c_float), ('bn_eps', C.c_float)]
 
 
+class OptimParams(C.Structure):
+    _fields_ = [('kind', C.c_int), ('momentum', C.c_double), ('dampening', C.c_double), ('weight_decay', C.c_double),
+                ('beta1', C.c_double), ('beta2', C.c_double), ('eps', C.c_double)]
+
+
 class OpInfo(C.Structure):
     _fields_ = [(n, C.c_int) for n in ('kind', 'in_', 'out', 'res', 'aux', 'in2', 'out2', 'stride', 'relu', 'heads', 'shift', 'level',
                                       'convd', 'out_mode', 'ext_proto', 'k', 'cin', 'cout', 'cout_pad', 'anchor_offset')] + \
@@ -156,6 +161,11 @@ PROTOTYPES = {
     'yb_train_backward': (C.c_int, [vp, vp, vp]),
     'yb_train_read': (C.c_int, [vp, C.c_char_p, C.c_int, vp, C.c_int64, C.POINTER(C.c_int), C.POINTER(C.c_int), vp]),
     'yb_train_launches_per_step': (C.c_uint64, [vp]),
+    'yb_optim_create': (C.c_int, [C.POINTER(OptimParams), C.c_int, C.POINTER(vp), C.POINTER(C.c_int64), C.POINTER(vp)]),
+    'yb_optim_step': (C.c_int, [vp, vp, C.c_double, C.c_float, vp]),
+    'yb_optim_read_state': (C.c_int, [vp, C.c_int, vp, C.c_int64, vp]),
+    'yb_optim_num_elements': (C.c_int64, [vp]),
+    'yb_optim_destroy': (None, [vp]),
 }
 
 _lib = None

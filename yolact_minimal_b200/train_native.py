@@ -98,9 +98,14 @@ class TrainEngine:
                        'yb_train_forward')
         return losses
 
-    def backward(self, loss_grad):
+    def backward_into_grad_flat(self, loss_grad=None):
+        """The backward pass of the last forward into `grad_flat` (overwritten); loss_grad None = ones."""
         with torch.cuda.device(self.device):
-            _lib.check(self.L.yb_train_backward(self.h, loss_grad.data_ptr(), torch.cuda.current_stream().cuda_stream), 'yb_train_backward')
+            _lib.check(self.L.yb_train_backward(self.h, None if loss_grad is None else loss_grad.data_ptr(),
+                                                torch.cuda.current_stream().cuda_stream), 'yb_train_backward')
+
+    def backward(self, loss_grad):
+        self.backward_into_grad_flat(loss_grad)
         return self.grad_flat.clone()                      # autograd may keep / alias what it is handed: never the engine's own buffer
 
     def read(self, name, grad=False):
@@ -147,8 +152,11 @@ class _NativeTrainStep(torch.autograd.Function):
         return (None,) * 8 + tuple(v.view_as(p) for v, p in zip(eng.grad_views(flat), eng._params))
 
 
-def training_step(net, img, box_classes, masks_gt):
-    """Yolact.forward in training mode: the reference's 4-tuple (category, box, mask, semantic) of losses."""
+def prepare_step(net, img, box_classes, masks_gt):
+    """The part of a training step before the engine runs: the engine for this batch size (created on first use and kept on the
+    module), its binding to the module's parameters and buffers, and the targets packed as yb_train_forward reads them.
+    Returns (engine, forward arguments, num_batches_tracked buffers).  Queues no host synchronisation when the targets are on
+    the device already: the gt offsets go through page-locked memory."""
     if not img.is_cuda:
         raise RuntimeError('yolact_minimal_b200.Yolact trains on CUDA only (no CPU fallback): move the model and input to the GPU')
     B, S = img.shape[0], net.cfg.img_size
@@ -176,12 +184,18 @@ def training_step(net, img, box_classes, masks_gt):
     counts = [int(t.shape[0]) for t in box_classes]
     gt = torch.cat([t.to(dev, torch.float32).reshape(-1, 5) for t in box_classes]).contiguous()
     masks = torch.cat([m.to(dev, torch.float32).reshape(-1, S, S) for m in masks_gt]).contiguous()
-    gt_off = torch.tensor(np.concatenate([[0], np.cumsum(counts)]).astype(np.int32), device=dev)
+    gt_off = torch.from_numpy(np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)).pin_memory().to(dev, non_blocking=True)
     if gt.shape[0] == 0:
         raise ValueError('training needs at least one ground-truth box in the batch')
     seed = int(torch.randint(0, 2 ** 31 - 1, (1,)).item())             # host RNG (like the reference's torch.randperm, yolact.py:263)
-    losses = _NativeTrainStep.apply(eng, img.detach().to(torch.float32).contiguous(), gt, gt_off, masks, int(gt.shape[0]), max(counts), seed,
-                                    *eng._params)
-    if cache[3]:
-        torch._foreach_add_(cache[3], 1)
+    args = (img.detach().to(torch.float32).contiguous(), gt, gt_off, masks, int(gt.shape[0]), max(counts), seed)
+    return eng, args, cache[3]
+
+
+def training_step(net, img, box_classes, masks_gt):
+    """Yolact.forward in training mode: the reference's 4-tuple (category, box, mask, semantic) of losses."""
+    eng, args, bns = prepare_step(net, img, box_classes, masks_gt)
+    losses = _NativeTrainStep.apply(eng, *args, *eng._params)
+    if bns:
+        torch._foreach_add_(bns, 1)
     return tuple(losses.unbind(0))
