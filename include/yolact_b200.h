@@ -192,6 +192,71 @@ YB_API int yb_eval_ap(const yb_eval_params* p, const float* rec_score, const int
                       const void* state, void* workspace, size_t workspace_bytes, double* ap, uint8_t* nonempty, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * COCO's own mAP: pycocotools' COCOeval (default Params, iouType 'bbox' and 'segm') for the detections of eval.py's loop, which
+ * --coco_api hands to pycocotools as JSON (eval.py:60-67,:78-98).  precision / recall equal COCOeval's float64 arrays bit for
+ * bit (DESIGN.md, COCO mAP on the GPU):
+ *   yb_cocoeval_match       per image: the detections the JSON would hold (class in range, (y2-y1)*(x2-x1) > 0), their rank
+ *                           within (image, class) by descending score (ties: detection order), the first max_dets[2] of each
+ *                           class kept; double IoUs against the image's gts of the same class (bbox: pycocotools' bbIou on xywh,
+ *                           crowd gts divide by the detection's area; segm: popcounts of the packed masks); then COCOeval's greedy
+ *                           matching for every slot (type, area range, IoU threshold).  Appends one record per kept detection
+ *                           in a region of count[b] records at the running count plus the earlier images' counts (no host sync);
+ *                           the unused tail of a region holds records of class -1.
+ *   yb_cocoeval_accumulate  COCOeval.accumulate: a stable sort of the records by (class, descending score, image rank), then
+ *                           per (type, IoU threshold, class, area range, maxDets) tp / fp counts in double, the running maximum
+ *                           of precision from the right sampled at searchsorted(recall, rec_thr, 'left').  precision
+ *                           [2][10][101][K][4][3] and recall [2][10][K][4][3] (type 0 = bbox, 1 = segm), -1 where npig = 0.
+ * Limits: max_det <= 256; bits(num_classes) + bits(num_images - 1) <= 32 (the sort key), e.g. 2^25 images at 80 classes.
+ * Inputs of yb_cocoeval_match (DEVICE pointers; batch B, max_det D, total_gt G):
+ *   count [B], cls [B,D] (0-based class), score [B,D], box_px [B,D,4] int32 x1,y1,x2,y2; det_masks / det_mask_off [B+1] (int64
+ *            words) / det_mask_words: at least count[b] packed masks of img_hw[b] = (h, w) per image, as yb_eval_match takes them
+ *   img_rank [B] int32: the image's position in ascending image-id order, 0 .. num_images-1
+ *   gt_cls [G] int32 (0-based class), gt_box [G,4] float64 x,y,w,h (the annotation's bbox), gt_area [G] float64 (its area),
+ *            gt_crowd [G] int32; gt_offset [B+1]: image b owns gts gt_offset[b] .. gt_offset[b+1], every annotation of the image
+ *            in file order, crowd included; gt_masks / gt_mask_off [B+1] / gt_mask_words: one packed mask per gt
+ *   state [yb_cocoeval_state_bytes]: zeroed before the first batch.  Bytes 0-7: records appended so far (uint64); bytes 12-15:
+ *            flags (bit 0: capacity exceeded, bit 1: an image's ranges lie outside the buffers or do not match its geometry,
+ *            bit 2: an image rank outside 0 .. num_images-1; such images append records of class -1).
+ * ---------------------------------------------------------------------------------------- */
+#define YB_COCOEVAL_THR 10
+#define YB_COCOEVAL_REC 101
+#define YB_COCOEVAL_AREAS 4
+#define YB_COCOEVAL_MAXDETS 3
+typedef struct {
+  int num_classes;                                /* K: len(catIds) */
+  int num_images;                                 /* len(imgIds) */
+  double iou_thr[YB_COCOEVAL_THR];                /* np.linspace(.5, .95, 10), made on the host */
+  double rec_thr[YB_COCOEVAL_REC];                /* np.linspace(0, 1, 101) */
+  double area_rng[YB_COCOEVAL_AREAS][2];          /* all / small / medium / large, both ends inclusive */
+  int max_dets[YB_COCOEVAL_MAXDETS];              /* 1, 10, 100 (ascending, at most 256) */
+} yb_cocoeval_params;
+
+typedef struct {
+  float score;
+  int32_t cls;                     /* 0-based class; -1: no detection */
+  int32_t img;                     /* image rank */
+  int16_t det;                     /* detection index in the image */
+  int16_t rank;                    /* rank within (image, class) */
+  uint32_t bits[8];                /* [type * 4 + area]: bit t matched at iou_thr[t], bit 16 + t ignored */
+} yb_cocoeval_record;
+
+YB_API size_t yb_cocoeval_state_bytes(void);
+YB_API size_t yb_cocoeval_match_workspace_bytes(int batch, int max_det, int64_t total_gt);
+YB_API int yb_cocoeval_match(const yb_cocoeval_params* p, int batch, int max_det, const int32_t* count, const int32_t* cls,
+                             const float* score, const int32_t* box_px, const uint32_t* det_masks, const int64_t* det_mask_off,
+                             int64_t det_mask_words, const int32_t* img_hw, const int32_t* img_rank, const int32_t* gt_cls,
+                             const double* gt_box, const double* gt_area, const int32_t* gt_crowd, const int32_t* gt_offset,
+                             int64_t total_gt, const uint32_t* gt_masks, const int64_t* gt_mask_off, int64_t gt_mask_words,
+                             yb_cocoeval_record* records, int64_t capacity, void* state, void* workspace, size_t workspace_bytes,
+                             void* stream);
+/* num_records: an upper bound of the records appended; npig [K][4] int64: non-ignored gts per (class, area range) over every image
+ * of the annotation set */
+YB_API size_t yb_cocoeval_accumulate_workspace_bytes(int64_t num_records);
+YB_API int yb_cocoeval_accumulate(const yb_cocoeval_params* p, const yb_cocoeval_record* records, int64_t num_records, const void* state,
+                                  const int64_t* npig, void* workspace, size_t workspace_bytes, double* precision, double* recall,
+                                  void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Pre-process -- replaces utils/augmentations.py:219-227 val_aug(img, val_size) (SURVEY.md 8(f) #1):
  * uint8 BGR HWC image [h,w,3] (device) -> float32 RGB CHW [3,S,S] (device): pad to square at the
  * top-left with the BGR mean, bilinear resize (OpenCV INTER_LINEAR coordinates), (x-mean)/std.

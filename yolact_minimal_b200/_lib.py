@@ -44,6 +44,18 @@ class EvalParams(C.Structure):
     _fields_ = [('num_classes', C.c_int), ('num_thr', C.c_int), ('thr', C.c_double * EVAL_MAX_THR)]
 
 
+COCOEVAL_THR, COCOEVAL_REC, COCOEVAL_AREAS, COCOEVAL_MAXDETS = 10, 101, 4, 3
+
+
+class CocoEvalParams(C.Structure):
+    _fields_ = [('num_classes', C.c_int), ('num_images', C.c_int), ('iou_thr', C.c_double * COCOEVAL_THR),
+                ('rec_thr', C.c_double * COCOEVAL_REC), ('area_rng', (C.c_double * 2) * COCOEVAL_AREAS),
+                ('max_dets', C.c_int * COCOEVAL_MAXDETS)]
+
+
+COCOEVAL_RECORD_BYTES = 48                 # sizeof(yb_cocoeval_record)
+
+
 class TrainHparams(C.Structure):
     _fields_ = [('pos_iou_thr', C.c_float), ('neg_iou_thr', C.c_float), ('neg_pos_ratio', C.c_int), ('masks_to_train', C.c_int),
                 ('conf_alpha', C.c_float), ('bbox_alpha', C.c_float), ('mask_alpha', C.c_float), ('semantic_alpha', C.c_float),
@@ -120,6 +132,12 @@ PROTOTYPES = {
     'yb_eval_match': (C.c_int, [C.POINTER(EvalParams), C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp, C.c_int64,
                                 vp, vp, C.c_int64, vp, vp, vp, C.c_int64, vp, vp, C.c_size_t, vp]),
     'yb_eval_ap': (C.c_int, [C.POINTER(EvalParams), vp, vp, vp, C.c_int64, vp, vp, C.c_size_t, vp, vp, vp]),
+    'yb_cocoeval_state_bytes': (C.c_size_t, []),
+    'yb_cocoeval_match_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int, C.c_int64]),
+    'yb_cocoeval_match': (C.c_int, [C.POINTER(CocoEvalParams), C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, C.c_int64, vp, vp, vp, vp,
+                                    vp, vp, vp, C.c_int64, vp, vp, C.c_int64, vp, C.c_int64, vp, vp, C.c_size_t, vp]),
+    'yb_cocoeval_accumulate_workspace_bytes': (C.c_size_t, [C.c_int64]),
+    'yb_cocoeval_accumulate': (C.c_int, [C.POINTER(CocoEvalParams), vp, C.c_int64, vp, vp, vp, C.c_size_t, vp, vp, vp]),
     'yb_net_create': (C.c_int, [C.POINTER(NetConfig), C.POINTER(vp)]),
     'yb_net_destroy': (None, [vp]),
     'yb_net_num_params': (C.c_int, [vp]),

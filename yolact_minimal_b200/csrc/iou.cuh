@@ -28,4 +28,23 @@ __device__ __forceinline__ float mask_iou_from_counts(const unsigned inter, cons
   return __fdiv_rn(fi, __fsub_rn(__fadd_rn((float)ca, (float)cb), fi));
 }
 
+// pycocotools' bbIou for one (detection, gt) pair of x,y,w,h boxes, in double with every operation separately rounded (no FMA
+// contraction): 0 when the overlap's width or height is <= 0; a crowd gt divides by the detection's area alone
+__device__ __forceinline__ double coco_box_iou(const double4 d, const double4 g, const bool crowd) {
+  const double w = __dsub_rn(fmin(__dadd_rn(d.x, d.z), __dadd_rn(g.x, g.z)), fmax(d.x, g.x));
+  if (w <= 0.0) return 0.0;
+  const double h = __dsub_rn(fmin(__dadd_rn(d.y, d.w), __dadd_rn(g.y, g.w)), fmax(d.y, g.y));
+  if (h <= 0.0) return 0.0;
+  const double i = __dmul_rn(w, h);
+  const double da = __dmul_rn(d.z, d.w);
+  const double u = crowd ? da : __dsub_rn(__dadd_rn(da, __dmul_rn(g.z, g.w)), i);
+  return __ddiv_rn(i, u);
+}
+
+// pycocotools' rleIou from the pixel counts, in double: 0 without overlap; a crowd gt divides by the detection's pixel count
+__device__ __forceinline__ double coco_mask_iou(const unsigned inter, const unsigned cd, const unsigned cg, const bool crowd) {
+  if (inter == 0) return 0.0;
+  return __ddiv_rn((double)inter, (double)(crowd ? cd : cd + cg - inter));
+}
+
 }  // namespace yb

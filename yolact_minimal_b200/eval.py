@@ -7,7 +7,9 @@ value `(table, box_row, mask_row)` and progress line, fed `cfg.val_bs` images at
 The rows equal the reference's per-image loop (eval.py:42-69,106 with val_aug, nms, after_nms, prep_metrics) bit for bit: the
 forward is batch-invariant, detect_batched treats images independently, after_nms_batched equals after_nms per image and
 MapEvaluator appends the images in order (DESIGN.md, batched evaluation).  With cfg.coco_api the detections go to MakeJson and
-pycocotools' COCOeval instead, as in the reference.
+pycocotools' COCOeval instead, as in the reference.  With cfg.coco_gpu (--coco_gpu) they go to utils.cocoeval.CocoEvaluator, which
+computes COCOeval's bbox and segm results on the GPU from the same detections, with no JSON and no COCOeval; evaluate() then
+prints COCOeval's two summaries and returns their stats (box_stats, mask_stats), float64 [12] each.
 
     python -m yolact_minimal_b200.eval --weight weights/best_30.5_res101_coco_392000.pth --val_bs 64
 """
@@ -21,6 +23,7 @@ from torch.utils.data import DataLoader
 from .utils import mask_utils
 from .utils.augmentations import val_aug_batch
 from .utils.coco import COCOValDetection, val_collate
+from .utils.cocoeval import CocoEvaluator
 from .utils.common_utils import APDataObject, MakeJson, ProgressBar, _bind, calc_map
 from .utils.output_utils import after_nms_batched, detect_batched
 
@@ -44,8 +47,12 @@ def _add_json(make_json, packed, det, boxes_px, masks):
 
 def evaluate(net, cfg, step=None, *, dataset=None, num_workers=4):
     """Box and mask mAP of `net` on COCO val (cfg.val_imgs / cfg.val_ann, cfg.val_num images), cfg.val_bs images per batch.
-    `dataset` replaces COCOValDetection(cfg) (any object with its item format), `num_workers` the loader's workers."""
-    dataset = COCOValDetection(cfg) if dataset is None else dataset
+    `dataset` replaces COCOValDetection(cfg) (any object with its item format; with cfg.coco_gpu, COCOValDetection's
+    coco_eval=True format and a `coco` attribute), `num_workers` the loader's workers."""
+    coco_gpu = bool(getattr(cfg, 'coco_gpu', False))
+    if coco_gpu and cfg.coco_api:
+        raise ValueError('evaluate: coco_api and coco_gpu are alternatives; set one')
+    dataset = COCOValDetection(cfg, coco_eval=coco_gpu) if dataset is None else dataset
     data_loader = DataLoader(dataset, int(cfg.val_bs), num_workers=num_workers, shuffle=False, pin_memory=True,
                              collate_fn=val_collate)
     ds = len(data_loader)
@@ -53,7 +60,8 @@ def evaluate(net, cfg, step=None, *, dataset=None, num_workers=4):
     dev = next(net.parameters()).device
     ap_data = {'box': [[APDataObject() for _ in cfg.class_names] for _ in iou_thres],
                'mask': [[APDataObject() for _ in cfg.class_names] for _ in iou_thres]}
-    evaluator = None if cfg.coco_api else _bind(ap_data, iou_thres, dev)
+    evaluator = None if cfg.coco_api or coco_gpu else _bind(ap_data, iou_thres, dev)
+    coco_ev = CocoEvaluator(dataset.coco, cfg.continuous_id, dev) if coco_gpu else None
     make_json = MakeJson() if cfg.coco_api else None
     start, seen = None, 0
     for i, packed in enumerate(data_loader):
@@ -66,6 +74,8 @@ def evaluate(net, cfg, step=None, *, dataset=None, num_workers=4):
         boxes_px, masks = after_nms_batched(det, proto_p, packed.sizes)
         if cfg.coco_api:
             _add_json(make_json, packed, det, boxes_px, masks)
+        elif coco_gpu:
+            coco_ev.add(det, boxes_px, masks, packed)
         else:
             gt, gt_masks = packed.gt_to(dev)
             evaluator.add(det, boxes_px, masks, gt, packed.gt_offset, gt_masks, packed.sizes)
@@ -75,6 +85,10 @@ def evaluate(net, cfg, step=None, *, dataset=None, num_workers=4):
             fps = seen / (time.perf_counter() - start)
             print(f'\rTesting: {progress_bar.get_bar(i + 1)} {i + 1}/{ds}, total fps: {fps:.2f}', end='')
 
+    if coco_gpu:
+        print()
+        box_stats, mask_stats = coco_ev.summarize()
+        return box_stats, mask_stats
     if cfg.coco_api:
         from pycocotools.coco import COCO
         from pycocotools.cocoeval import COCOeval
@@ -111,13 +125,18 @@ def main(argv=None):
     parser.add_argument('--traditional_nms', default=False, action='store_true', help='Whether to use traditional nms.')
     parser.add_argument('--val_num', default=-1, type=int, help='The number of images for test, set to -1 for all.')
     parser.add_argument('--coco_api', action='store_true', help='Whether to use cocoapi to evaluate results.')
+    parser.add_argument('--coco_gpu', action='store_true', help='Compute COCOeval\'s box and mask mAP on the GPU (no JSON, '
+                        'no pycocotools for the metric).')
     parser.add_argument('--val_bs', default=1, type=int, help='Images per batch on the GPU.')
     args = parser.parse_args(argv)
+    if args.coco_api and args.coco_gpu:
+        parser.error('--coco_api and --coco_gpu are alternatives')
     prefix = re.findall(r'best_\d+\.\d+_', args.weight)[0]
     suffix = re.findall(r'_\d+\.pth', args.weight)[0]
     args.cfg = args.weight.split(prefix)[-1].split(suffix)[0]
     cfg = get_config(args, mode='val')
     cfg.val_bs = args.val_bs
+    cfg.coco_gpu = args.coco_gpu
     if cfg.coco_api:
         make_output_dirs()
 

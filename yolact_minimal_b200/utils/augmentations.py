@@ -89,14 +89,20 @@ class PackedValBatch:
       gt_masks         torch int32: every image's packed gt masks [g_b, h_b, ceil(w_b/32)] back to back; gt_mask_off [B+1] (words)
       sizes, ids       (h, w) and the COCO image id of every image
     It is built in DataLoader workers (utils.coco.val_collate) and holds only picklable types; with DataLoader(pin_memory=True)
-    the loader's pin thread calls pin_memory() and the copies to the device are asynchronous."""
+    the loader's pin thread calls pin_memory() and the copies to the device are asynchronous.
+    Samples of COCOValDetection(..., coco_eval=True) also fill what CocoEvaluator.add needs, every annotation of every image:
+      ann_cls int32 [N], ann_box float64 [N,4] (x,y,w,h), ann_area float64 [N], ann_crowd int32 [N]; ann_offset [B+1]
+      ann_masks        torch int32: the annotations' packed masks back to back; ann_mask_off [B+1] (words)
+    Otherwise these stay None."""
+
+    ann_cls = ann_box = ann_area = ann_crowd = ann_offset = ann_masks = ann_mask_off = None
 
     def __init__(self, samples):
-        """samples: list of (img_u8 [h,w,3], gt float32 [g,5], gt_bits int32 [g,h,ceil(w/32)], (h, w), image id)."""
+        """samples: list of (img_u8 [h,w,3], gt float32 [g,5], gt_bits int32 [g,h,ceil(w/32)], (h, w), image id[, annotations])."""
         self.buffer, self.items = pack_images([s[0] for s in samples])
         self.sizes = [(int(s[3][0]), int(s[3][1])) for s in samples]
         self.ids = [s[4] for s in samples]
-        for i, (img, gt, bits, (h, w), _) in enumerate(samples):
+        for i, (img, gt, bits, (h, w), _) in enumerate(s[:5] for s in samples):
             if img.shape[:2] != (h, w) or gt.dtype != np.float32 or gt.ndim != 2 or gt.shape[1] != 5 or bits.dtype != np.int32 or \
                     bits.shape != (gt.shape[0], h, (w + 31) // 32):
                 raise ValueError(f'sample {i}: image {img.shape}, gt {gt.dtype} {gt.shape} and gt masks {bits.dtype} {bits.shape} do not '
@@ -105,13 +111,32 @@ class PackedValBatch:
         self.gt_mask_off = np.concatenate([[0], np.cumsum([s[2].size for s in samples])]).astype(int).tolist()
         self.gt = torch.from_numpy(np.concatenate([s[1] for s in samples]).reshape(-1, 5))
         self.gt_masks = torch.from_numpy(np.concatenate([s[2].reshape(-1) for s in samples]))
+        if samples and all(len(s) > 5 for s in samples):
+            self._pack_annotations([s[5] for s in samples])
+
+    def _pack_annotations(self, anns):
+        for i, ((cls, box, area, crowd, bits), (h, w)) in enumerate(zip(anns, self.sizes)):
+            m = len(cls)
+            if cls.dtype != np.int32 or box.dtype != np.float64 or box.shape != (m, 4) or area.dtype != np.float64 or \
+                    area.shape != (m,) or crowd.dtype != np.int32 or crowd.shape != (m,) or bits.dtype != np.int32 or \
+                    bits.shape != (m, h, (w + 31) // 32):
+                raise ValueError(f'sample {i}: annotation tables {cls.shape} {box.shape} {area.shape} {crowd.shape} {bits.shape} do not '
+                                 f'describe {m} annotations of one {h}x{w} image')
+        self.ann_offset = np.concatenate([[0], np.cumsum([len(a[0]) for a in anns])]).astype(int).tolist()
+        self.ann_mask_off = np.concatenate([[0], np.cumsum([a[4].size for a in anns])]).astype(int).tolist()
+        self.ann_cls, self.ann_box, self.ann_area, self.ann_crowd, self.ann_masks = (
+            torch.from_numpy(np.concatenate([a[j].reshape((-1, 4) if j == 1 else -1) for a in anns])) for j in range(5))
 
     def __len__(self):
         return len(self.items)
 
     def pin_memory(self):
-        """Called by DataLoader(pin_memory=True) in its pin thread: page-locks the images, the gts and the gt masks."""
+        """Called by DataLoader(pin_memory=True) in its pin thread: page-locks the images, the gts and the gt masks (and the
+        annotation tables when there are any)."""
         self.buffer, self.gt, self.gt_masks = self.buffer.pin_memory(), self.gt.pin_memory(), self.gt_masks.pin_memory()
+        if self.ann_cls is not None:
+            self.ann_cls, self.ann_box, self.ann_area, self.ann_crowd, self.ann_masks = (
+                t.pin_memory() for t in (self.ann_cls, self.ann_box, self.ann_area, self.ann_crowd, self.ann_masks))
         return self
 
     def gt_to(self, device):

@@ -89,7 +89,7 @@ class COCODetection:
 
 
 def val_collate(batch):
-    """Packs a batch of COCOValDetection samples for val_aug_batch and MapEvaluator.add."""
+    """Packs a batch of COCOValDetection samples for val_aug_batch and MapEvaluator.add (or CocoEvaluator.add)."""
     return PackedValBatch(batch)
 
 
@@ -101,10 +101,16 @@ class COCOValDetection:
 
     Returns (img_u8 [h,w,3] BGR, gt float32 [n,5], gt masks bit-packed int32 [n,h,ceil(w/32)] (mask_utils.pack_masks layout),
     (h, w), COCO image id); val_aug runs on the device for a whole batch.  `coco` may be passed in (any object with the
-    pycocotools.coco.COCO methods used here); by default it is pycocotools' COCO on cfg.val_ann."""
+    pycocotools.coco.COCO methods used here); by default it is pycocotools' COCO on cfg.val_ann.
 
-    def __init__(self, cfg, coco=None):
+    With coco_eval=True each sample also carries every annotation of the image in file order, crowd ones included, for
+    utils.cocoeval.CocoEvaluator: (class int32 [m] (continuous_id - 1), bbox float64 [m,4] (the annotation's x,y,w,h), area
+    float64 [m], iscrowd int32 [m], masks bit-packed int32 [m,h,ceil(w/32)] (annToMask)).  The images visited, their order, len()
+    and the RuntimeError rule stay the same."""
+
+    def __init__(self, cfg, coco=None, coco_eval=False):
         self.cfg = cfg
+        self.coco_eval = bool(coco_eval)
         self.image_path = cfg.val_imgs
         if coco is None:
             from pycocotools.coco import COCO
@@ -121,18 +127,26 @@ class COCOValDetection:
 
     def __getitem__(self, index):
         img_id = self.ids[index]
-        target = [a for a in self.coco.loadAnns(self.coco.getAnnIds(imgIds=img_id)) if not a['iscrowd']]
+        anns = self.coco.loadAnns(self.coco.getAnnIds(imgIds=img_id))
+        target = [a for a in anns if not a['iscrowd']]
         img = self.load_image(self.coco.loadImgs(img_id)[0]['file_name'])
         height, width, _ = img.shape
         if not target:
             raise RuntimeError('Error, no valid object in this image.')
         boxes = np.array([[a['bbox'][0], a['bbox'][1], a['bbox'][0] + a['bbox'][2], a['bbox'][1] + a['bbox'][3]] for a in target])
         labels = np.array([self.continuous_id[a['category_id']] - 1 for a in target])
-        masks = np.stack([self.coco.annToMask(a) for a in target], axis=0)
+        all_masks = [self.coco.annToMask(a) for a in (anns if self.coco_eval else target)]
+        masks = np.stack([m for m, a in zip(all_masks, anns) if not a['iscrowd']] if self.coco_eval else all_masks, axis=0)
         assert masks.shape == (boxes.shape[0], height, width), 'Unmatched annotations.'
         boxes = boxes / np.array([width, height, width, height])
         gt = np.hstack((boxes, np.expand_dims(labels, axis=1))).astype(np.float32)
-        return np.ascontiguousarray(img), gt, pack_masks_host(masks), (height, width), img_id
+        sample = (np.ascontiguousarray(img), gt, pack_masks_host(masks), (height, width), img_id)
+        if not self.coco_eval:
+            return sample
+        ann = (np.array([self.continuous_id[a['category_id']] - 1 for a in anns], np.int32),
+               np.array([a['bbox'] for a in anns], np.float64).reshape(-1, 4), np.array([a['area'] for a in anns], np.float64),
+               np.array([int(a['iscrowd']) for a in anns], np.int32), pack_masks_host(np.stack(all_masks, axis=0)))
+        return sample + (ann,)
 
 
 class PackedDetectBatch:
