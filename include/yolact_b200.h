@@ -277,6 +277,21 @@ YB_API int yb_val_aug_batch(const uint8_t* src, int64_t src_bytes, const yb_val_
                             void* workspace, size_t workspace_bytes, float* out, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * JPEG encoding -- cv2.imwrite / cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, quality]) of uint8 BGR images, byte for
+ * byte: baseline, 4:2:0, ISLOW DCT, Annex K Huffman tables, JFIF header, no restart markers (oracle/jpeg_np.py).
+ * src and items as yb_val_aug_batch (items is a HOST table, images of any sizes).  out_off is a HOST array of n + 1 byte offsets
+ * into the device buffer out: file i is written at out[out_off[i] ..) and its length to out_len[i] (device); out_off[i+1] -
+ * out_off[i] must be at least yb_jpeg_encode_bound(h, w).  No byte of out past out_off[i] + out_len[i] changes.  Every offset,
+ * size and the quality (1 .. 100) are checked on the host before anything is launched (YB_ERR_INVALID); the tables then go
+ * through the page-locked staging, so the call queues on the stream without waiting: five launches, no synchronisation.
+ * ---------------------------------------------------------------------------------------- */
+YB_API int64_t yb_jpeg_encode_bound(int h, int w);   /* worst-case file bytes of an h x w image (-1 outside 1 .. 65535) */
+YB_API size_t yb_jpeg_encode_workspace_bytes(const yb_val_aug_item* items, int n);
+YB_API int yb_jpeg_encode_batch(const uint8_t* src, int64_t src_bytes, const yb_val_aug_item* items, int n, int quality,
+                                void* workspace, size_t workspace_bytes, uint8_t* out, const int64_t* out_off, int64_t* out_len,
+                                void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Training augmentation -- the pixel work of utils/augmentations.py:230-252 train_aug for a batch, given the
  * plans drawn on the host by yolact_minimal_b200.utils.augmentations.train_aug_plan (every random draw of
  * train_aug depends only on shapes and boxes, so the host keeps them and the device only moves pixels).

@@ -11,6 +11,10 @@ ends after the last write).  For each det_bs, a separate instrumented pass times
 limit read in the same run) and writes it to --out.
 
     python tools/bench_detect.py [--images 256] [--frames 64] [--out profiles/h100_bench_detect.json]
+
+With --jpeg_gpu it runs the image arms only, at det_bs 8 and 32, both with cv2.imwrite and with detect --jpeg_gpu (images/s end to
+end), and splits the host pass of a batch into the cv2 labels and the encode: cv2.imencode of each drawn image, or the JpegWriter's
+packing and queueing (mean ms per batch).  Its default --out is profiles/h100_bench_detect_jpeg.json.
 """
 import argparse
 import glob
@@ -87,12 +91,79 @@ def stage_times(net, cfg, packed_batches):
     return {s: round(v / n, 4) for s, v in acc.items()}, round(host_ms / n, 3)
 
 
+def host_split(net, cfg, batches):
+    """Mean ms per batch of the host pass: cv2 labels (finish with the device already done), then the encode of the drawn
+    images: cv2.imencode each, or JpegWriter.put_host + flush (packing into page-locked memory and queueing the encode)."""
+    import cv2
+    hosts = (yd._HostBuffers(), yd._HostBuffers())
+    labels, cv2_enc, gpu_enc = [], [], []
+    writer = yd.JpegWriter()
+    for i, packed in enumerate(batches):
+        p = yd.enqueue(net, cfg, packed, hosts[i % 2])
+        torch.cuda.synchronize()
+        drawn = []
+        t0 = time.perf_counter()
+        yd.finish(p, cfg, lambda name, img: drawn.append((name, img.copy())))
+        labels.append(time.perf_counter() - t0)
+        t0 = time.perf_counter()
+        for _, img in drawn:
+            cv2.imencode('.jpg', img)
+        cv2_enc.append(time.perf_counter() - t0)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        for name, img in drawn:
+            writer.put_host(f'results/images/{name}', img)
+        writer.flush()
+        gpu_enc.append(time.perf_counter() - t0)
+    writer.close()
+    ms = lambda v: round(1e3 * float(np.mean(v[1:])), 3)
+    return {'labels_ms': ms(labels), 'cv2_encode_ms': ms(cv2_enc), 'jpeg_gpu_queue_ms': ms(gpu_enc)}
+
+
+def jpeg_arm(args, net, cfg, rng):
+    import cv2
+    result = {'gpu': torch.cuda.get_device_name(0), 'power_limit_w': power_limit(), 'model': 'res101_coco 550 fp16, synthetic weights',
+              'visual_thre': 0.3, 'images': args.images}
+    with tempfile.TemporaryDirectory() as tmp:
+        folder = os.path.join(tmp, 'images')
+        os.makedirs(folder)
+        for k in range(args.images):
+            cv2.imwrite(os.path.join(folder, f'{k:04d}.jpg'), scene(k, *SIZES[k % len(SIZES)], rng))
+        os.chdir(tmp)
+        os.makedirs('results/images')
+        cfg.image = folder
+        for jpeg_gpu in (False, True):                                             # warm-up
+            cfg.jpeg_gpu = jpeg_gpu
+            yd.detect_images(net, cfg, 32)
+        e2e = {}
+        for bs in (8, 32):
+            for jpeg_gpu in (False, True):
+                cfg.jpeg_gpu = jpeg_gpu
+                t0 = time.perf_counter()
+                yd.detect_images(net, cfg, bs)
+                e2e[f'det_bs{bs}' + ('_jpeg_gpu' if jpeg_gpu else '')] = round(args.images / (time.perf_counter() - t0), 2)
+        cfg.jpeg_gpu = False
+        result['images_per_s'] = e2e
+        ds = DetectImages(cfg)
+        split = {}
+        for bs in (8, 32):
+            batches = [detect_collate([ds[i] for i in range(j, min(j + bs, len(ds)))]).pin_memory()
+                       for j in range(0, min(len(ds), 9 * bs), bs)]
+            split[f'det_bs{bs}'] = host_split(net, cfg, batches)
+        result['host_pass_ms_per_batch'] = split
+        os.chdir(ROOT)
+    return result
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--images', type=int, default=256)
     ap.add_argument('--frames', type=int, default=64)
-    ap.add_argument('--out', default=os.path.join(ROOT, 'profiles', 'h100_bench_detect.json'))
+    ap.add_argument('--jpeg_gpu', action='store_true')
+    ap.add_argument('--out', default=None)
     args = ap.parse_args()
+    if args.out is None:
+        args.out = os.path.join(ROOT, 'profiles', 'h100_bench_detect_jpeg.json' if args.jpeg_gpu else 'h100_bench_detect.json')
     import cv2
     dev = torch.device('cuda')
     cfg = make_config('res101_coco', 550, mode='detect', visual_thre=0.3)
@@ -101,6 +172,13 @@ def main():
     net.load_state_dict(ft.synth_state_dict('res101', seed=0), strict=True)
     net = net.to(dev).eval()
     rng = np.random.RandomState(5)
+    if args.jpeg_gpu:
+        result = jpeg_arm(args, net, cfg, rng)
+        line = json.dumps(result)
+        print(line)
+        with open(args.out, 'w') as f:
+            f.write(line + '\n')
+        return
     result = {'gpu': torch.cuda.get_device_name(0), 'power_limit_w': power_limit(), 'model': 'res101_coco 550 fp16, synthetic weights',
               'visual_thre': 0.3, 'images': args.images, 'frames': args.frames}
     with tempfile.TemporaryDirectory() as tmp:

@@ -114,7 +114,11 @@ PROTOTYPES = {
     'yb_val_aug': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, vp, vp]),
     'yb_val_aug_batch_workspace_bytes': (C.c_size_t, [C.c_int]),
     'yb_val_aug_batch': (C.c_int, [vp, C.c_int64, vp, C.c_int, C.c_int, vp, C.c_size_t, vp, vp]),
-    'yb_train_aug_workspace_bytes': (C.c_size_t, [C.c_int, C.c_int64]),
+    'yb_jpeg_encode_bound': (C.c_int64, [C.c_int, C.c_int]),
+    'yb_jpeg_encode_workspace_bytes': (C.c_size_t, [C.POINTER(ValAugItem), C.c_int]),
+    'yb_jpeg_encode_batch': (C.c_int, [vp, C.c_int64, C.POINTER(ValAugItem), C.c_int, C.c_int, vp, C.c_size_t, vp,
+                                       C.POINTER(C.c_int64), vp, vp]),
+    'yb_train_aug_workspace_bytes':(C.c_size_t, [C.c_int, C.c_int64]),
     'yb_train_aug': (C.c_int, [vp, C.c_int64, C.POINTER(TrainAugItem), C.c_int, vp, C.c_int, vp, C.c_size_t, vp, vp, vp]),
     'yb_pack_mask_bits': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),
     'yb_mask_iou_bits': (C.c_int, [vp, C.c_int, vp, C.c_int, C.c_int64, vp, vp]),

@@ -6,6 +6,9 @@ lincomb_{name}, the cutout images, results/videos/{name}), fed `--det_bs` images
     draw_labels (cv2 boxes, labels, fps) -> cv2.imwrite / VideoWriter.write                                  (host, one batch behind)
 
 The host waits for batch i only after batch i+1 is queued, so the cv2 pass of one batch runs under the device work of the next.
+With --jpeg_gpu the image files are encoded on the device (yb_jpeg_encode_batch, the bytes cv2.imwrite writes): the drawn images
+of a batch go into one page-locked buffer, one H2D copy, one encode and one D2H copy on a stream of their own, and the files are
+written one batch later; lincomb_{name} and the cutout images are encoded where they are, on the device.
 Every written image equals the reference's per-image loop (val_aug, net, nms, after_nms, draw_img) on this package bit for bit:
 the forward is batch-invariant at a fixed max_batch, detect_batched treats images independently, visual_thre keeps a prefix of
 each image's score-sorted detections, after_nms_batched equals after_nms per image and bit-packed masks draw as float masks do.
@@ -18,11 +21,12 @@ import time
 
 import torch
 
+from . import _lib
 from .utils.augmentations import val_aug_batch
 from .utils.coco import DetectImages, PackedDetectBatch, detect_collate
 from .utils.common_utils import ProgressBar
-from .utils.output_utils import (after_nms_batched, blend_masks_batched, cutout_masks, detect_batched, draw_labels, lincomb_batched,
-                                 visible_count)
+from .utils.output_utils import (after_nms_batched, blend_masks_batched, cutout_masks, cutout_masks_device, detect_batched, draw_labels,
+                                 imencode_batched, lincomb_batched, visible_count)
 
 
 class _HostBuffers:
@@ -39,6 +43,75 @@ class _HostBuffers:
         buf = buf[:t.numel()]
         buf.copy_(t.reshape(-1), non_blocking=True)
         return buf.view(t.shape)
+
+
+class JpegWriter:
+    """Writes JPEG files encoded on the device, byte for byte what cv2.imwrite(path, img) writes.  A batch's files are collected
+    with put_host (host images: packed into one page-locked buffer) and put_device (images already on the device), then flush(after)
+    queues their encodes on the writer's own stream behind the event `after`, with one D2H copy per encode, and writes the previous
+    batch's files.  close() writes the last batch's."""
+
+    def __init__(self, quality=95):
+        self.quality = quality
+        self.stream = torch.cuda.Stream()
+        self._host, self._device, self._pending = [], [], None
+
+    def put_host(self, path, img):
+        self._host.append((path, img))
+
+    def put_device(self, paths, buffer, items, keep=None):
+        """paths[i] receives image items[i] (yb_val_aug_item layout) of the CUDA uint8 `buffer`; `keep` (e.g. the tensors a kernel
+        queued on the writer's stream reads) is held until the files are written."""
+        self._device.append((list(paths), buffer, items, keep))
+
+    def _encode(self, paths, buffer, items, keep):
+        data, off, lengths = imencode_batched(buffer, items, self.quality)
+        data_h = torch.empty(data.numel(), dtype=torch.uint8, pin_memory=True)
+        len_h = torch.empty(lengths.numel(), dtype=torch.int64, pin_memory=True)
+        data_h.copy_(data, non_blocking=True)
+        len_h.copy_(lengths, non_blocking=True)
+        return paths, off, data_h, len_h, (data, buffer, keep)
+
+    def flush(self, after=None):
+        import numpy as np
+        from .utils.augmentations import VAL_ITEM_DTYPE
+        jobs = []
+        with torch.cuda.stream(self.stream):
+            if after is not None:
+                self.stream.wait_event(after)
+            if self._host:
+                items = np.zeros(len(self._host), VAL_ITEM_DTYPE)
+                buf = torch.empty(sum(img.nbytes for _, img in self._host), dtype=torch.uint8, pin_memory=True)
+                flat, o = buf.numpy(), 0
+                for i, (_, img) in enumerate(self._host):
+                    flat[o:o + img.nbytes] = np.ascontiguousarray(img).reshape(-1)
+                    items[i] = (o, img.shape[0], img.shape[1])
+                    o += img.nbytes
+                src = buf.to(torch.cuda.current_device(), non_blocking=True)
+                jobs.append(self._encode([p for p, _ in self._host], src, items, buf))
+            for paths, buffer, items, keep in self._device:
+                jobs.append(self._encode(paths, buffer, items, keep))
+            done = torch.cuda.Event()
+            done.record()
+        self._host, self._device = [], []
+        self._write()
+        self._pending = (jobs, done)
+
+    def _write(self):
+        if self._pending is None:
+            return
+        jobs, done = self._pending
+        done.synchronize()
+        for paths, off, data_h, len_h, _ in jobs:
+            data, lens = data_h.numpy(), len_h.numpy()
+            for i, path in enumerate(paths):
+                with open(path, 'wb') as f:
+                    f.write(data[off[i]:off[i] + lens[i]].tobytes())
+        self._pending = None
+
+    def close(self):
+        self.flush()
+        self._write()
 
 
 class _Pending:
@@ -61,18 +134,40 @@ def enqueue(net, cfg, packed, host):
     out = {'count': det['count'], 'cls': det['cls'], 'score': det['score'], 'boxes': boxes_px}
     if not cfg.hide_mask:
         out['frames'] = blend_masks_batched(src, packed.items, det, masks, cfg.num_classes)
+    lincomb = None
     if cfg.save_lincomb:
-        out['lincomb'] = lincomb_batched(proto_p, det)
+        lincomb = lincomb_batched(proto_p, det)
+        if not getattr(cfg, 'jpeg_gpu', False):
+            out['lincomb'] = lincomb
+            lincomb = None
     res = {k: host.take(k, v) for k, v in out.items()}
     done = torch.cuda.Event()
     done.record()
-    return _Pending(packed=packed, src=src, det=det, masks=masks, res=res, done=done)
+    return _Pending(packed=packed, src=src, det=det, masks=masks, res=res, done=done, lincomb=lincomb)
 
 
-def finish(p, cfg, emit, fps=None):
+def _put_cutouts(writer, p, b, n, boxes_np, cfg):
+    """The cutout images of image b, cut and encoded on the writer's stream without leaving the device."""
+    import numpy as np
+    from .utils.augmentations import VAL_ITEM_DTYPE
+    h, w = p.packed.sizes[b]
+    off, name = int(p.packed.items[b]['img_off']), p.packed.names[b]
+    with torch.cuda.stream(writer.stream):
+        writer.stream.wait_event(p.done)
+        src_b = p.src[off:off + h * w * 3].view(h, w, 3)
+        total, crops, coff, shapes = cutout_masks_device(src_b, p.det['cls'][b, :n], boxes_np, p.masks[b][:n], cfg.num_classes)
+    writer.put_device([f'results/images/{name}_total_obj.jpg'], total.view(-1), np.array([(0, h, w)], VAL_ITEM_DTYPE), keep=p)
+    if shapes:
+        items = np.array([(coff[i], ch, cw) for i, (ch, cw) in enumerate(shapes)], VAL_ITEM_DTYPE)
+        writer.put_device([f'results/images/{name}_{i}.jpg' for i in range(len(shapes))], crops, items)
+
+
+def finish(p, cfg, emit, fps=None, writer=None):
     """Waits for a queued batch and runs the host pass of draw_img on each image: lincomb_{name} (save_lincomb), the cutout images,
-    then the boxes / labels / fps; emit(name, image) receives each drawn image."""
+    then the boxes / labels / fps; emit(name, image) receives each drawn image.  With a JpegWriter the lincomb and cutout images
+    are encoded on the device and the writer is flushed after the batch."""
     import cv2
+    import numpy as np
     p.done.synchronize()
     r, packed = p.res, p.packed
     count = r['count'].numpy()
@@ -81,14 +176,20 @@ def finish(p, cfg, emit, fps=None):
         if n <= 0:                                        # after_nms returned None: draw_img gives back img_origin
             emit(name, packed.image(b))
             continue
-        if cfg.save_lincomb:
+        if cfg.save_lincomb and writer is not None:
+            _, H, W, _ = p.lincomb.shape
+            writer.put_device([f'results/images/lincomb_{name}'], p.lincomb.view(-1),
+                              np.array([(b * H * W * 3, H, W)], np.dtype(_lib.ValAugItem)))
+        elif cfg.save_lincomb:
             cv2.imwrite(f'results/images/lincomb_{name}', r['lincomb'][b].numpy())
         ids_np, scores_np, boxes_np = r['cls'][b, :n].numpy(), r['score'][b, :n].numpy(), r['boxes'][b, :n].numpy()
         if cfg.hide_mask:
             img = packed.image(b)                         # drawn in place, as the reference draws into img_origin
         else:
             off = int(packed.items[b]['img_off'])
-            if cfg.cutout:
+            if cfg.cutout and writer is not None:
+                _put_cutouts(writer, p, b, n, boxes_np, cfg)
+            elif cfg.cutout:
                 src_b = p.src[off:off + h * w * 3].view(h, w, 3)
                 total, crops = cutout_masks(src_b, p.det['cls'][b, :n], boxes_np, p.masks[b][:n], cfg.num_classes)
                 cv2.imwrite(f'results/images/{name}_total_obj.jpg', total)
@@ -96,9 +197,11 @@ def finish(p, cfg, emit, fps=None):
                     cv2.imwrite(f'results/images/{name}_{i}.jpg', crop)
             img = r['frames'][off:off + h * w * 3].numpy().reshape(h, w, 3)
         emit(name, draw_labels(img, ids_np, scores_np, boxes_np, cfg, fps))
+    if writer is not None:
+        writer.flush(p.done)
 
 
-def run(net, cfg, batches, emit, progress=None):
+def run(net, cfg, batches, emit, progress=None, writer=None):
     """Detects every batch of `batches` (PackedDetectBatch) with one batch in flight while the host draws the previous one.
     progress(done_images, images_per_second) is called after each batch; the rate is also the fps the real_time view shows."""
     hosts = (_HostBuffers(), _HostBuffers())
@@ -106,14 +209,14 @@ def run(net, cfg, batches, emit, progress=None):
     for i, packed in enumerate(batches):
         cur = enqueue(net, cfg, packed, hosts[i % 2])
         if pending is not None:
-            finish(pending, cfg, emit, fps)
+            finish(pending, cfg, emit, fps, writer)
             done += len(pending.packed)
             fps = done / (time.perf_counter() - start)
             if progress:
                 progress(done, fps)
         pending = cur
     if pending is not None:
-        finish(pending, cfg, emit, fps)
+        finish(pending, cfg, emit, fps, writer)
         done += len(pending.packed)
         if progress:
             progress(done, done / (time.perf_counter() - start))
@@ -131,7 +234,12 @@ def detect_images(net, cfg, det_bs, num_workers=2):
     def progress(done, fps):
         print(f'\rTesting: {bar.get_bar(done)} {done}/{len(dataset)}, total fps: {fps:.2f}', end='')
 
-    run(net, cfg, loader, lambda name, img: cv2.imwrite(f'results/images/{name}', img), progress)
+    if getattr(cfg, 'jpeg_gpu', False):
+        writer = JpegWriter()
+        run(net, cfg, loader, lambda name, img: writer.put_host(f'results/images/{name}', img), progress, writer)
+        writer.close()
+    else:
+        run(net, cfg, loader, lambda name, img: cv2.imwrite(f'results/images/{name}', img), progress)
     print('\nFinished, saved in: results/images.')
 
 
@@ -198,6 +306,8 @@ def main(argv=None):
     parser.add_argument('--visual_thre', default=0.3, type=float,
                         help='Detections with a score under this threshold will be removed.')
     parser.add_argument('--det_bs', default=1, type=int, help='Images (or video frames) per batch on the GPU.')
+    parser.add_argument('--jpeg_gpu', default=False, action='store_true',
+                        help='Encode the image files on the GPU (the same bytes cv2.imwrite writes).')
     args = parser.parse_args(argv)
     if args.det_bs < 1:
         parser.error(f'--det_bs must be >= 1, got {args.det_bs}')

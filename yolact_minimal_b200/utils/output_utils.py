@@ -410,6 +410,15 @@ def cutout_masks(img, ids, boxes, masks, num_classes):
     """draw_img's cfg.cutout images (utils/output_utils.py:328-341) on the device.  Returns (total_obj [h,w,3], [crop_i]) as host
     uint8 arrays: total_obj = img where the semantic index is non-zero, else 255; crop_i = (img where masks_i, else 255)[y1:y2,
     x1:x2] with numpy's slicing of the int box (x1, y1, x2, y2) = boxes[i] (a host array)."""
+    total, crops, off, shapes = cutout_masks_device(img, ids, boxes, masks, num_classes)
+    flat = crops.cpu().numpy()
+    out = [flat[off[i]:off[i + 1]].reshape(*shapes[i], 3) for i in range(len(shapes))]
+    return total.cpu().numpy(), out
+
+
+def cutout_masks_device(img, ids, boxes, masks, num_classes):
+    """cutout_masks without the copies to the host: (total_obj, crops, offsets, shapes) with total_obj a CUDA uint8 [h,w,3], crops
+    a CUDA uint8 buffer holding crop_i at bytes offsets[i] .. offsets[i+1] (host int64), and shapes[i] its (height, width)."""
     import numpy as np
     img, ids32, m, fmt, h, w = _draw_operands(img, ids, masks)
     n = int(ids32.shape[0])
@@ -430,9 +439,7 @@ def cutout_masks(img, ids, boxes, masks, num_classes):
     with torch.cuda.device(dev):
         _lib.check(L.yb_draw_cutout(img.data_ptr(), h, w, m.data_ptr(), fmt, n, ids32.data_ptr(), nc, yyxx_d.data_ptr(), off_d.data_ptr(),
                                     total.data_ptr(), crops.data_ptr(), torch.cuda.current_stream().cuda_stream), 'yb_draw_cutout')
-    flat = crops.cpu().numpy()
-    out = [flat[off[i]:off[i + 1]].reshape(yyxx[i, 1] - yyxx[i, 0], yyxx[i, 3] - yyxx[i, 2], 3) for i in range(n)]
-    return total.cpu().numpy(), out
+    return total, crops, off, [(int(yyxx[i, 1] - yyxx[i, 0]), int(yyxx[i, 3] - yyxx[i, 2])) for i in range(n)]
 
 
 def draw_img(ids_p, class_p, box_p, mask_p, img_origin, cfg, img_name=None, fps=None):
@@ -497,3 +504,60 @@ def draw_labels(img_fused, ids_np, scores_np, boxes_np, cfg, fps=None):
         img_fused = img_fused.astype(np.uint8)
         cv2.putText(img_fused, fps_str, (0, text_h + 2), font, scale, (255, 255, 255), thickness, cv2.LINE_AA)
     return img_fused
+
+
+# ---- JPEG encoding on the device (yb_jpeg_encode_batch): the bytes cv2.imencode('.jpg', img, [IMWRITE_JPEG_QUALITY, q]) returns
+def jpeg_bound(h, w):
+    """Worst-case size in bytes of the JPEG file of an h x w image (yb_jpeg_encode_bound)."""
+    b = int(_lib.lib().yb_jpeg_encode_bound(int(h), int(w)))
+    if b < 0:
+        raise ValueError(f'no JPEG of a {h}x{w} image (1 .. 65535 each)')
+    return b
+
+
+def imencode_batched(buffer, items, quality=95):
+    """cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality]) for a batch of images on the device, in one
+    yb_jpeg_encode_batch call queued on the current stream (no host synchronisation).  `buffer` is a CUDA uint8 tensor holding
+    uint8 BGR HWC images, `items` their numpy table in yb_val_aug_item's layout (augmentations.pack_images).
+    Returns (data, offsets, lengths): data a CUDA uint8 tensor, offsets a host int64 array [n + 1], lengths a CUDA int64 tensor
+    [n]; file i is data[offsets[i]:offsets[i] + lengths[i]]."""
+    import numpy as np
+    _require_cuda(buffer)
+    if buffer.dtype != torch.uint8 or buffer.dim() != 1 or not buffer.is_contiguous():
+        raise ValueError('buffer must be a contiguous 1-D uint8 tensor')
+    items = np.ascontiguousarray(items, dtype=np.dtype(_lib.ValAugItem))
+    n = len(items)
+    if n == 0:
+        raise ValueError('no images to encode')
+    offsets = np.zeros(n + 1, np.int64)
+    offsets[1:] = np.cumsum([jpeg_bound(h, w) for h, w in zip(items['h'], items['w'])])
+    L = _lib.lib()
+    item_p = items.ctypes.data_as(ctypes.POINTER(_lib.ValAugItem))
+    dev = buffer.device
+    with torch.cuda.device(dev):
+        ws_bytes = int(L.yb_jpeg_encode_workspace_bytes(item_p, n))
+        ws = torch.empty(max(ws_bytes, 1), dtype=torch.uint8, device=dev)
+        data = torch.empty(int(offsets[-1]), dtype=torch.uint8, device=dev)
+        lengths = torch.empty(n, dtype=torch.int64, device=dev)
+        _lib.check(L.yb_jpeg_encode_batch(buffer.data_ptr(), buffer.numel(), item_p, n, int(quality), ws.data_ptr(), ws_bytes,
+                                          data.data_ptr(), offsets.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), lengths.data_ptr(),
+                                          torch.cuda.current_stream().cuda_stream), 'yb_jpeg_encode_batch')
+    return data, offsets, lengths
+
+
+def imencode_gpu(img, quality=95):
+    """cv2.imencode('.jpg', img, [cv2.IMWRITE_JPEG_QUALITY, quality])[1] for one uint8 BGR image [h, w, 3] (numpy, or a CUDA
+    tensor), encoded on the device: a 1-D numpy uint8 array of the file's bytes."""
+    import numpy as np
+    if isinstance(img, torch.Tensor):
+        t = img.detach()
+        if not t.is_cuda:
+            t = t.cuda()
+    else:
+        t = torch.from_numpy(np.ascontiguousarray(img)).cuda()
+    if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3:
+        raise ValueError(f'expected a uint8 HxWx3 BGR image, got {t.dtype} {tuple(t.shape)}')
+    h, w = int(t.shape[0]), int(t.shape[1])
+    items = np.array([(0, h, w)], dtype=np.dtype(_lib.ValAugItem))
+    data, _, lengths = imencode_batched(t.contiguous().reshape(-1), items, quality)
+    return data[:int(lengths[0])].cpu().numpy()
