@@ -292,6 +292,30 @@ YB_API int yb_jpeg_encode_batch(const uint8_t* src, int64_t src_bytes, const yb_
                                 void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * JPEG decoding -- cv2.imread(path) of a batch of JPEG files, pixel for pixel: libjpeg-turbo's ISLOW IDCT, fancy upsampling,
+ * BGR output, then the EXIF orientation applied as OpenCV applies it (oracle/jpeg_decode_np.py).  Supported files: baseline or
+ * extended-sequential Huffman, 8-bit, one scan holding every component, with or without restart intervals; grayscale, or YCbCr
+ * with chroma 1x1 and luma 1x1, 2x1 or 2x2 (4:4:4, 4:2:2, 4:2:0).
+ *
+ * Host only: reads the markers of one file.  YB_OK with the output h, w (orientation applied) for a supported file,
+ * YB_ERR_UNSUPPORTED for a valid JPEG outside the supported set, YB_ERR_INVALID for a malformed header. */
+YB_API int yb_jpeg_header(const uint8_t* data, int64_t len, int32_t* h, int32_t* w);
+/* File i is src[src_off[i] .. src_off[i+1]) (src_off a HOST array of n + 1 offsets), in both a HOST copy src_host (for the
+ * headers) and a device copy src_dev (for the entropy-coded data).  Image i is written as uint8 BGR [h,w,3] at out + items[i].img_off
+ * (items a HOST yb_val_aug_item table, the layout yb_val_aug_batch reads).  Headers, sizes against items and offsets are checked on
+ * the host before anything is launched (YB_ERR_INVALID / YB_ERR_UNSUPPORTED, what yb_jpeg_header returns); the tables then go
+ * through the page-locked staging, so the call queues without waiting: five launches, no synchronisation.
+ * status (device int32 [n]): 0 for a clean decode; nonzero for corrupt entropy-coded data (an invalid code, a run past coefficient
+ * 63, the wrong number of restart markers, too few blocks).  A corrupt stream never reads outside its file nor writes outside
+ * its output slot; what the slot then holds is unspecified.  After the call the first n int32 of the workspace hold each file's
+ * number of synchronisation rounds of the Huffman decode (0 for a file whose restart markers are wrong).
+ * yb_jpeg_decode_workspace_bytes returns 0 if a header does not parse. */
+YB_API size_t yb_jpeg_decode_workspace_bytes(const uint8_t* src_host, const int64_t* src_off, int n);
+YB_API int yb_jpeg_decode_batch(const uint8_t* src_host, const uint8_t* src_dev, const int64_t* src_off, int n,
+                                const yb_val_aug_item* items, uint8_t* out, int64_t out_bytes,
+                                void* workspace, size_t workspace_bytes, int32_t* status, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Training augmentation -- the pixel work of utils/augmentations.py:230-252 train_aug for a batch, given the
  * plans drawn on the host by yolact_minimal_b200.utils.augmentations.train_aug_plan (every random draw of
  * train_aug depends only on shapes and boxes, so the host keeps them and the device only moves pixels).

@@ -15,6 +15,11 @@ limit read in the same run) and writes it to --out.
 With --jpeg_gpu it runs the image arms only, at det_bs 8 and 32, both with cv2.imwrite and with detect --jpeg_gpu (images/s end to
 end), and splits the host pass of a batch into the cv2 labels and the encode: cv2.imencode of each drawn image, or the JpegWriter's
 packing and queueing (mean ms per batch).  Its default --out is profiles/h100_bench_detect_jpeg.json.
+
+With --decode_gpu it runs the image arms only, at det_bs 8 and 32 with 2 loader workers (detect's default): cv2.imread in the
+workers against detect --decode_gpu, each with cv2.imwrite and with --jpeg_gpu (images/s end to end), and what one worker does per
+image to read it (cv2.imread, or np.fromfile plus yb_jpeg_header; median ms on one thread).  Its default --out is
+profiles/h100_bench_detect_decode.json.
 """
 import argparse
 import glob
@@ -155,15 +160,49 @@ def jpeg_arm(args, net, cfg, rng):
     return result
 
 
+def decode_arm(args, net, cfg, rng):
+    import cv2
+    from bench_val import read_ms
+    result = {'gpu': torch.cuda.get_device_name(0), 'power_limit_w': power_limit(), 'model': 'res101_coco 550 fp16, synthetic weights',
+              'visual_thre': 0.3, 'images': args.images, 'workers': 2, 'files': 'cv2.imwrite defaults (q95, 4:2:0)'}
+    with tempfile.TemporaryDirectory() as tmp:
+        folder = os.path.join(tmp, 'images')
+        os.makedirs(folder)
+        for k in range(args.images):
+            cv2.imwrite(os.path.join(folder, f'{k:04d}.jpg'), scene(k, *SIZES[k % len(SIZES)], rng))
+        result['worker_read_ms_per_image'] = read_ms(sorted(glob.glob(os.path.join(folder, '*.jpg')))[:64])
+        os.chdir(tmp)
+        os.makedirs('results/images')
+        cfg.image = folder
+        for decode_gpu in (False, True):                                           # warm-up
+            cfg.decode_gpu = decode_gpu
+            yd.detect_images(net, cfg, 32)
+        e2e = {}
+        for bs in (8, 32):
+            for jpeg_gpu in (False, True):
+                for decode_gpu in (False, True):
+                    cfg.jpeg_gpu, cfg.decode_gpu = jpeg_gpu, decode_gpu
+                    t0 = time.perf_counter()
+                    yd.detect_images(net, cfg, bs)
+                    key = f'det_bs{bs}' + ('_jpeg_gpu' if jpeg_gpu else '') + ('_decode_gpu' if decode_gpu else '')
+                    e2e[key] = round(args.images / (time.perf_counter() - t0), 2)
+        cfg.jpeg_gpu = cfg.decode_gpu = False
+        result['images_per_s'] = e2e
+        os.chdir(ROOT)
+    return result
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--images', type=int, default=256)
     ap.add_argument('--frames', type=int, default=64)
     ap.add_argument('--jpeg_gpu', action='store_true')
+    ap.add_argument('--decode_gpu', action='store_true')
     ap.add_argument('--out', default=None)
     args = ap.parse_args()
     if args.out is None:
-        args.out = os.path.join(ROOT, 'profiles', 'h100_bench_detect_jpeg.json' if args.jpeg_gpu else 'h100_bench_detect.json')
+        args.out = os.path.join(ROOT, 'profiles', 'h100_bench_detect_decode.json' if args.decode_gpu else
+                                'h100_bench_detect_jpeg.json' if args.jpeg_gpu else 'h100_bench_detect.json')
     import cv2
     dev = torch.device('cuda')
     cfg = make_config('res101_coco', 550, mode='detect', visual_thre=0.3)
@@ -172,8 +211,8 @@ def main():
     net.load_state_dict(ft.synth_state_dict('res101', seed=0), strict=True)
     net = net.to(dev).eval()
     rng = np.random.RandomState(5)
-    if args.jpeg_gpu:
-        result = jpeg_arm(args, net, cfg, rng)
+    if args.decode_gpu or args.jpeg_gpu:
+        result = decode_arm(args, net, cfg, rng) if args.decode_gpu else jpeg_arm(args, net, cfg, rng)
         line = json.dumps(result)
         print(line)
         with open(args.out, 'w') as f:

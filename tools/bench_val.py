@@ -11,6 +11,12 @@ Both arms end in calc_map; their (box_row, mask_row) must be identical.  Prints 
 the same run) and writes it to --out.
 
     python tools/bench_val.py [--images 1024] [--batch 64] [--out profiles/h100_bench_val.json]
+
+With --decode_gpu it instead times evaluate(net, cfg) end to end on the same images written as JPEG files (cv2.imwrite: q95,
+4:2:0) with a stub COCO of their gts, 4 loader workers as evaluate's default: once with cv2.imread in the workers and once with
+--decode_gpu (the workers read the files' bytes, each batch is decoded on the device).  Images/s by the host clock around the
+whole call, after a warm-up call of each; the rows of both must be identical.  It also times what one worker does per image to
+read it (cv2.imread, or np.fromfile plus yb_jpeg_header).  Its default --out is profiles/h100_bench_val_decode.json.
 """
 import argparse
 import json
@@ -116,18 +122,90 @@ def batched(net, cfg, batches, dev, events=None):
     return ap_data
 
 
+def read_ms(paths):
+    """Median ms per image, on one thread, of what a worker does to read an image: cv2.imread, or the bytes and the header."""
+    import cv2
+    from yolact_minimal_b200.utils.augmentations import read_image
+    cv2.setNumThreads(1)
+    out = {}
+    for key, fn in (('cv2_imread', cv2.imread), ('decode_gpu_read', lambda p: read_image(p, decode_gpu=True))):
+        ts = []
+        for p in paths:
+            t0 = time.perf_counter()
+            fn(p)
+            ts.append(time.perf_counter() - t0)
+        out[key] = round(1e3 * float(np.median(ts)), 3)
+    return out
+
+
+def decode_arm(a, net, cfg, dev):
+    import tempfile
+    import cv2
+    from test_val_batch_gpu import _StubCOCO
+    from yolact_minimal_b200.config import COCO_LABEL_MAP
+    from yolact_minimal_b200.eval import evaluate
+    from yolact_minimal_b200.utils.coco import COCOValDetection
+    coco_id = {label - 1: cid for cid, label in COCO_LABEL_MAP.items()}
+    items = samples(net, cfg, images(a.images), a.batch, dev)
+    res = dict(bench='bench_val --decode_gpu', gpu=torch.cuda.get_device_name(0), power_limit_w=power_limit(), arch='res101_coco',
+               img_size=550, precision='fp16', val_bs=a.batch, images=a.images, sizes=[list(s) for s in SIZES], workers=4,
+               files='cv2.imwrite defaults (q95, 4:2:0)')
+    with tempfile.TemporaryDirectory() as tmp:
+        meta, nbytes = {}, 0
+        for k, (img, gt, _, (h, w), _) in enumerate(items):
+            name = f'{k:05d}.jpg'
+            cv2.imwrite(os.path.join(tmp, name), img)
+            nbytes += os.path.getsize(os.path.join(tmp, name))
+            anns = []
+            for row in gt.astype(np.float64):
+                x1, y1, x2, y2 = row[:4] * [w, h, w, h]
+                anns.append(dict(bbox=[x1, y1, x2 - x1, y2 - y1], category_id=coco_id[int(row[4])], iscrowd=0, _hw=(h, w)))
+            meta[k] = (name, h, w, anns)
+        res['file_mb'] = round(nbytes / 1e6, 2)
+        res['pixel_mb'] = round(sum(it[0].nbytes for it in items) / 1e6, 2)
+        res['worker_read_ms_per_image'] = read_ms([os.path.join(tmp, meta[k][0]) for k in range(min(64, len(meta)))])
+        coco = _StubCOCO(meta)
+        cfg.val_imgs, cfg.val_bs, cfg.val_num = tmp, a.batch, -1
+        rows, ips = {}, {}
+        for decode_gpu in (False, True):
+            cfg.decode_gpu = decode_gpu
+            ds = COCOValDetection(cfg, coco=coco, decode_gpu=decode_gpu)
+            evaluate(net, cfg, dataset=ds)                                 # warm-up: workers, engine, workspaces
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            rows[decode_gpu] = evaluate(net, cfg, dataset=ds)
+            torch.cuda.synchronize()
+            ips['decode_gpu' if decode_gpu else 'cv2_imread'] = round(a.images / (time.perf_counter() - t0), 1)
+        cfg.decode_gpu = False
+    assert rows[True] == rows[False], (rows[True][1:], rows[False][1:])
+    assert rows[False][1][1] > 0, 'the workload has no matches: the row comparison would be vacuous'
+    res.update(images_per_s_end_to_end=ips, rows_equal=True, box_row=rows[False][1], mask_row=rows[False][2],
+               batched_gpu_images_per_s='profiles/h100_bench_val.json')
+    return res
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--images', type=int, default=1024)
     ap.add_argument('--batch', type=int, default=64)
-    ap.add_argument('--out', default=os.path.join(ROOT, 'profiles', 'h100_bench_val.json'))
+    ap.add_argument('--decode_gpu', action='store_true')
+    ap.add_argument('--out', default=None)
     a = ap.parse_args()
+    if a.out is None:
+        a.out = os.path.join(ROOT, 'profiles', 'h100_bench_val_decode.json' if a.decode_gpu else 'h100_bench_val.json')
     dev = torch.device('cuda:0')
     cfg = make_config('res101_coco', 550, mode='val')
     cfg.precision, cfg.max_batch = 'fp16', a.batch
     net = Yolact(cfg)
     net.load_state_dict(ft.synth_state_dict('res101', seed=0), strict=True)
     net = net.to(dev).eval()
+    if a.decode_gpu:
+        line = json.dumps(decode_arm(a, net, cfg, dev))
+        print(line)
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, 'w') as f:
+            f.write(line + '\n')
+        return
     items = samples(net, cfg, images(a.images), a.batch, dev)
     batches = [PackedValBatch(items[i:i + a.batch]).pin_memory() for i in range(0, len(items), a.batch)]
 

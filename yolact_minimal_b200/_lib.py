@@ -118,6 +118,10 @@ PROTOTYPES = {
     'yb_jpeg_encode_workspace_bytes': (C.c_size_t, [C.POINTER(ValAugItem), C.c_int]),
     'yb_jpeg_encode_batch': (C.c_int, [vp, C.c_int64, C.POINTER(ValAugItem), C.c_int, C.c_int, vp, C.c_size_t, vp,
                                        C.POINTER(C.c_int64), vp, vp]),
+    'yb_jpeg_header': (C.c_int, [vp, C.c_int64, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    'yb_jpeg_decode_workspace_bytes': (C.c_size_t, [vp, C.POINTER(C.c_int64), C.c_int]),
+    'yb_jpeg_decode_batch': (C.c_int, [vp, vp, C.POINTER(C.c_int64), C.c_int, C.POINTER(ValAugItem), vp, C.c_int64, vp, C.c_size_t,
+                                       vp, vp]),
     'yb_train_aug_workspace_bytes':(C.c_size_t, [C.c_int, C.c_int64]),
     'yb_train_aug': (C.c_int, [vp, C.c_int64, C.POINTER(TrainAugItem), C.c_int, vp, C.c_int, vp, C.c_size_t, vp, vp, vp]),
     'yb_pack_mask_bits': (C.c_int, [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp]),

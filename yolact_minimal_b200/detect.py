@@ -9,6 +9,9 @@ The host waits for batch i only after batch i+1 is queued, so the cv2 pass of on
 With --jpeg_gpu the image files are encoded on the device (yb_jpeg_encode_batch, the bytes cv2.imwrite writes): the drawn images
 of a batch go into one page-locked buffer, one H2D copy, one encode and one D2H copy on a stream of their own, and the files are
 written one batch later; lincomb_{name} and the cutout images are encoded where they are, on the device.
+With --decode_gpu the loader's workers read the files' bytes instead of decoding them, and a batch's JPEG files are decoded on the
+device (yb_jpeg_decode_batch, the pixels cv2.imread returns) in place of the H2D copy of its pixels; files it refuses are read by
+cv2.imread in the workers as before.  A file with corrupt entropy-coded data raises once its batch has run.
 Every written image equals the reference's per-image loop (val_aug, net, nms, after_nms, draw_img) on this package bit for bit:
 the forward is batch-invariant at a fixed max_batch, detect_batched treats images independently, visual_thre keeps a prefix of
 each image's score-sorted detections, after_nms_batched equals after_nms per image and bit-packed masks draw as float masks do.
@@ -124,7 +127,8 @@ class _Pending:
 def enqueue(net, cfg, packed, host):
     """Queues one batch's device work and the copies of its results into `host` (a _HostBuffers); never waits for the device."""
     dev = next(net.parameters()).device
-    src = packed.buffer.to(dev, non_blocking=packed.buffer.is_pinned())
+    decoded = packed.buffer is None
+    src, status = packed.to_device(dev)
     with torch.no_grad():
         images = val_aug_batch(src, packed.items, cfg.img_size, dev)
         class_p, box_p, coef_p, proto_p = net(images)
@@ -140,7 +144,13 @@ def enqueue(net, cfg, packed, host):
         if not getattr(cfg, 'jpeg_gpu', False):
             out['lincomb'] = lincomb
             lincomb = None
+    if decoded:
+        out['pixels'] = src                               # the host pass draws on (and emits) the decoded pixels
+        if status is not None:
+            out['status'] = status
     res = {k: host.take(k, v) for k, v in out.items()}
+    if decoded:
+        packed.buffer = res['pixels']
     done = torch.cuda.Event()
     done.record()
     return _Pending(packed=packed, src=src, det=det, masks=masks, res=res, done=done, lincomb=lincomb)
@@ -170,6 +180,10 @@ def finish(p, cfg, emit, fps=None, writer=None):
     import numpy as np
     p.done.synchronize()
     r, packed = p.res, p.packed
+    if 'status' in r:
+        bad = [packed.names[int(packed.mixed.encoded[k])] for k in np.flatnonzero(r['status'].numpy())]
+        if bad:
+            raise RuntimeError(f'corrupt JPEG data in {", ".join(str(b) for b in bad)}')
     count = r['count'].numpy()
     for b, (h, w) in enumerate(packed.sizes):
         n, name = int(count[b]), packed.names[b]
@@ -226,7 +240,7 @@ def detect_images(net, cfg, det_bs, num_workers=2):
     """The reference's image loop (detect.py:52-99): every cfg.image/*.jpg, drawn to results/images/{name}."""
     import cv2
     from torch.utils.data import DataLoader
-    dataset = DetectImages(cfg)
+    dataset = DetectImages(cfg, decode_gpu=getattr(cfg, 'decode_gpu', False))
     assert len(dataset) > 0, 'No .jpg images found.'
     loader = DataLoader(dataset, det_bs, num_workers=num_workers, shuffle=False, pin_memory=True, collate_fn=detect_collate)
     bar = ProgressBar(40, len(dataset))
@@ -308,6 +322,8 @@ def main(argv=None):
     parser.add_argument('--det_bs', default=1, type=int, help='Images (or video frames) per batch on the GPU.')
     parser.add_argument('--jpeg_gpu', default=False, action='store_true',
                         help='Encode the image files on the GPU (the same bytes cv2.imwrite writes).')
+    parser.add_argument('--decode_gpu', default=False, action='store_true',
+                        help='Decode the input JPEG files on the GPU (the same pixels cv2.imread returns).')
     args = parser.parse_args(argv)
     if args.det_bs < 1:
         parser.error(f'--det_bs must be >= 1, got {args.det_bs}')

@@ -9,7 +9,9 @@ forward is batch-invariant, detect_batched treats images independently, after_nm
 MapEvaluator appends the images in order (DESIGN.md, batched evaluation).  With cfg.coco_api the detections go to MakeJson and
 pycocotools' COCOeval instead, as in the reference.  With cfg.coco_gpu (--coco_gpu) they go to utils.cocoeval.CocoEvaluator, which
 computes COCOeval's bbox and segm results on the GPU from the same detections, with no JSON and no COCOeval; evaluate() then
-prints COCOeval's two summaries and returns their stats (box_stats, mask_stats), float64 [12] each.
+prints COCOeval's two summaries and returns their stats (box_stats, mask_stats), float64 [12] each.  With cfg.decode_gpu
+(--decode_gpu) the workers read the JPEG files' bytes and each batch is decoded on the device (yb_jpeg_decode_batch, the pixels
+cv2.imread returns); the decode statuses are read once at the end, and a file with corrupt entropy-coded data raises.
 
     python -m yolact_minimal_b200.eval --weight weights/best_30.5_res101_coco_392000.pth --val_bs 64
 """
@@ -17,6 +19,7 @@ import argparse
 import re
 import time
 
+import numpy as np
 import torch
 from torch.utils.data import DataLoader
 
@@ -52,7 +55,8 @@ def evaluate(net, cfg, step=None, *, dataset=None, num_workers=4):
     coco_gpu = bool(getattr(cfg, 'coco_gpu', False))
     if coco_gpu and cfg.coco_api:
         raise ValueError('evaluate: coco_api and coco_gpu are alternatives; set one')
-    dataset = COCOValDetection(cfg, coco_eval=coco_gpu) if dataset is None else dataset
+    decode_gpu = bool(getattr(cfg, 'decode_gpu', False))
+    dataset = COCOValDetection(cfg, coco_eval=coco_gpu, decode_gpu=decode_gpu) if dataset is None else dataset
     data_loader = DataLoader(dataset, int(cfg.val_bs), num_workers=num_workers, shuffle=False, pin_memory=True,
                              collate_fn=val_collate)
     ds = len(data_loader)
@@ -64,11 +68,18 @@ def evaluate(net, cfg, step=None, *, dataset=None, num_workers=4):
     coco_ev = CocoEvaluator(dataset.coco, cfg.continuous_id, dev) if coco_gpu else None
     make_json = MakeJson() if cfg.coco_api else None
     start, seen = None, 0
+    statuses = []                                 # (device status, image ids of its entries) of the batches decoded on the device
     for i, packed in enumerate(data_loader):
         if i == 1:
             start, seen = time.perf_counter(), 0
         with torch.no_grad():
-            images = val_aug_batch(packed.buffer, packed.items, cfg.img_size, dev)
+            if packed.mixed is not None:
+                buffer, status = packed.to_device(dev)
+                if status is not None:
+                    statuses.append((status, [packed.ids[int(k)] for k in packed.mixed.encoded]))
+            else:
+                buffer = packed.buffer
+            images = val_aug_batch(buffer, packed.items, cfg.img_size, dev)
             class_p, box_p, coef_p, proto_p = net(images)
         det = detect_batched(class_p, box_p, coef_p, net.anchors, cfg)
         boxes_px, masks = after_nms_batched(det, proto_p, packed.sizes)
@@ -85,6 +96,12 @@ def evaluate(net, cfg, step=None, *, dataset=None, num_workers=4):
             fps = seen / (time.perf_counter() - start)
             print(f'\rTesting: {progress_bar.get_bar(i + 1)} {i + 1}/{ds}, total fps: {fps:.2f}', end='')
 
+    if statuses:
+        codes = torch.cat([s for s, _ in statuses]).cpu().numpy()
+        ids = [i for _, b in statuses for i in b]
+        bad = [ids[k] for k in np.flatnonzero(codes)]
+        if bad:
+            raise RuntimeError(f'corrupt JPEG data in the images with ids {bad}')
     if coco_gpu:
         print()
         box_stats, mask_stats = coco_ev.summarize()
@@ -128,6 +145,8 @@ def main(argv=None):
     parser.add_argument('--coco_gpu', action='store_true', help='Compute COCOeval\'s box and mask mAP on the GPU (no JSON, '
                         'no pycocotools for the metric).')
     parser.add_argument('--val_bs', default=1, type=int, help='Images per batch on the GPU.')
+    parser.add_argument('--decode_gpu', action='store_true', help='Decode the JPEG files on the GPU (the same pixels cv2.imread '
+                        'returns).')
     args = parser.parse_args(argv)
     if args.coco_api and args.coco_gpu:
         parser.error('--coco_api and --coco_gpu are alternatives')
@@ -137,6 +156,7 @@ def main(argv=None):
     cfg = get_config(args, mode='val')
     cfg.val_bs = args.val_bs
     cfg.coco_gpu = args.coco_gpu
+    cfg.decode_gpu = args.decode_gpu
     if cfg.coco_api:
         make_output_dirs()
 

@@ -59,6 +59,148 @@ def pack_images(images):
     return torch.from_numpy(buf), items
 
 
+# ----------------------------------------------------------------------------- JPEG decoding on the device
+def jpeg_header(data):
+    """(h, w) cv2.imread would return for the JPEG file bytes `data` (orientation applied) when yb_jpeg_decode_batch decodes it,
+    None for a file it refuses (progressive, arithmetic, CMYK, 4:1:1, 4:4:0, not a JPEG ...; cv2.imread reads those)."""
+    data = np.ascontiguousarray(data, dtype=np.uint8)
+    h, w = C.c_int32(), C.c_int32()
+    if _lib.lib().yb_jpeg_header(data.ctypes.data, data.size, C.byref(h), C.byref(w)) != 0:
+        return None
+    return int(h.value), int(w.value)
+
+
+class EncodedImage:
+    """A JPEG file's bytes (numpy uint8) and the (h, w) yb_jpeg_header read from them: what a DataLoader worker returns instead of
+    the pixels when the batch is decoded on the device."""
+
+    __slots__ = ('data', 'h', 'w')
+
+    def __init__(self, data, h, w):
+        self.data, self.h, self.w = data, int(h), int(w)
+
+    @property
+    def shape(self):
+        return (self.h, self.w, 3)
+
+    @property
+    def nbytes(self):
+        return self.h * self.w * 3
+
+
+def read_image(path, decode_gpu=False):
+    """cv2.imread(path); with decode_gpu, the file's bytes as an EncodedImage when yb_jpeg_header accepts them (cv2.imread
+    otherwise).  None when cv2 cannot read the file either."""
+    if decode_gpu:
+        data = np.fromfile(path, np.uint8)
+        hw = jpeg_header(data)
+        if hw is not None:
+            return EncodedImage(data, *hw)
+    import cv2
+    return cv2.imread(path)
+
+
+def imdecode_batched(files_host, src_off, items, device='cuda', out=None):
+    """Decodes JPEG files on the device: file i is files_host[src_off[i]:src_off[i+1]] (a torch uint8 CPU tensor, page-locked for
+    an asynchronous copy) and lands as uint8 BGR [h,w,3] at byte items[i]['img_off'] of the device buffer (yb_val_aug_item
+    table; `out`, or a new buffer just large enough).  One H2D copy of the file bytes and one yb_jpeg_decode_batch, no host sync.
+    Returns (buffer, status): status a device int32 [n], nonzero where the entropy-coded data is corrupt."""
+    device = torch.device(device)
+    if device.type != 'cuda':
+        raise _lib.YolactB200Error('imdecode_batched runs on a CUDA device (no CPU fallback)')
+    if isinstance(files_host, np.ndarray):
+        files_host = torch.from_numpy(np.ascontiguousarray(files_host, dtype=np.uint8))
+    items = np.ascontiguousarray(items, dtype=VAL_ITEM_DTYPE)
+    src_off = np.ascontiguousarray(src_off, dtype=np.int64)
+    n = len(items)
+    if len(src_off) != n + 1:
+        raise ValueError(f'src_off must hold {n + 1} offsets, got {len(src_off)}')
+    L = _lib.lib()
+    host = files_host.numpy()
+    off_p = src_off.ctypes.data_as(C.POINTER(C.c_int64))
+    ws_bytes = int(L.yb_jpeg_decode_workspace_bytes(host.ctypes.data, off_p, n))
+    if ws_bytes == 0:
+        raise _lib.YolactB200Error('imdecode_batched: a file is not a JPEG yb_jpeg_decode_batch decodes (see yb_jpeg_header)')
+    need = int(max((int(o) + int(h) * int(w) * 3 for o, h, w in items.tolist()), default=0))
+    with torch.cuda.device(device):
+        stream = torch.cuda.current_stream()
+        src = files_host.to(device, non_blocking=files_host.is_pinned())
+        if out is None:
+            out = torch.empty(max(need, 1), dtype=torch.uint8, device=device)
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        status = torch.empty(n, dtype=torch.int32, device=device)
+        _lib.check(L.yb_jpeg_decode_batch(host.ctypes.data, src.data_ptr(), off_p, n, items.ctypes.data_as(C.POINTER(_lib.ValAugItem)),
+                                          out.data_ptr(), out.numel(), ws.data_ptr(), ws_bytes, status.data_ptr(), stream.cuda_stream),
+                   'yb_jpeg_decode_batch')
+    return out, status
+
+
+def imread_gpu(path, device='cuda'):
+    """cv2.imread(path) as a CUDA uint8 tensor [h,w,3]: decoded on the device by yb_jpeg_decode_batch, or by cv2 for a file it
+    refuses.  Raises RuntimeError if the file cannot be read or its entropy-coded data is corrupt."""
+    img = read_image(path, decode_gpu=True)
+    if img is None:
+        raise RuntimeError(f'cannot read image {path}')
+    if not isinstance(img, EncodedImage):
+        return torch.from_numpy(np.ascontiguousarray(img)).to(device)
+    items = np.array([(0, img.h, img.w)], VAL_ITEM_DTYPE)
+    out, status = imdecode_batched(torch.from_numpy(img.data), [0, img.data.size], items, device)
+    if int(status[0]) != 0:
+        raise RuntimeError(f'corrupt JPEG data in {path}')
+    return out.view(img.h, img.w, 3)
+
+
+class MixedImages:
+    """A batch of images as JPEG file bytes (EncodedImage) and, for the files decoded by cv2, raw uint8 BGR pixels.  `items` is
+    the yb_val_aug_item table of the device buffer to_device() fills, in pack_images' layout."""
+
+    def __init__(self, images):
+        self.items = np.zeros(len(images), dtype=VAL_ITEM_DTYPE)
+        enc = [i for i, im in enumerate(images) if isinstance(im, EncodedImage)]
+        raw = [i for i, im in enumerate(images) if not isinstance(im, EncodedImage)]
+        off = 0
+        for i, im in enumerate(images):
+            if not isinstance(im, EncodedImage) and (im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3):
+                raise ValueError(f'image {i}: expected a uint8 HxWx3 BGR image, got {im.dtype} {im.shape}')
+            self.items[i] = (off, im.shape[0], im.shape[1])
+            off += im.nbytes
+        self.nbytes = off
+        self.encoded = np.array(enc, np.int64)
+        self.file_off = np.concatenate([[0], np.cumsum([images[i].data.size for i in enc])]).astype(np.int64)
+        self.files = torch.from_numpy(np.concatenate([images[i].data for i in enc]) if enc else np.zeros(1, np.uint8))
+        self.raw = [(int(self.items[i]['img_off']), images[i].nbytes) for i in raw]
+        self.pixels = torch.from_numpy(np.concatenate([images[i].reshape(-1) for i in raw]) if raw else np.zeros(1, np.uint8))
+
+    def pin_memory(self):
+        self.files, self.pixels = self.files.pin_memory(), self.pixels.pin_memory()
+        return self
+
+    def to_device(self, device):
+        """-> (CUDA uint8 buffer holding every image in `items`' layout, device int32 status of the decoded files (index
+        self.encoded[k] for entry k), or None when no file is decoded on the device).  No host sync."""
+        device = torch.device(device)
+        out = torch.empty(max(self.nbytes, 1), dtype=torch.uint8, device=device)
+        status = None
+        if len(self.encoded):
+            _, status = imdecode_batched(self.files, self.file_off, self.items[self.encoded], device, out=out)
+        if self.raw:
+            px = self.pixels.to(device, non_blocking=self.pixels.is_pinned())
+            o = 0
+            for dst, n in self.raw:
+                out[dst:dst + n].copy_(px[o:o + n], non_blocking=True)
+                o += n
+        return out, status
+
+
+def pack_any(images):
+    """pack_images for a batch that may hold EncodedImages: (buffer, items, None) without any, (None, items, MixedImages) with."""
+    if any(isinstance(im, EncodedImage) for im in images):
+        mixed = MixedImages(images)
+        return None, mixed.items, mixed
+    buf, items = pack_images(images)
+    return buf, items, None
+
+
 def val_aug_batch(buffer, items, val_size, device='cuda'):
     """val_aug for a batch: `buffer` a torch uint8 tensor holding B BGR HWC images back to back, `items` their numpy table
     (pack_images).  One H2D copy of the buffer (asynchronous when it is pinned), one yb_val_aug_batch launch.
@@ -97,9 +239,12 @@ class PackedValBatch:
 
     ann_cls = ann_box = ann_area = ann_crowd = ann_offset = ann_masks = ann_mask_off = None
 
+    mixed = None
+
     def __init__(self, samples):
-        """samples: list of (img_u8 [h,w,3], gt float32 [g,5], gt_bits int32 [g,h,ceil(w/32)], (h, w), image id[, annotations])."""
-        self.buffer, self.items = pack_images([s[0] for s in samples])
+        """samples: list of (img_u8 [h,w,3] or EncodedImage, gt float32 [g,5], gt_bits int32 [g,h,ceil(w/32)], (h, w), image
+        id[, annotations]).  With EncodedImages `buffer` is None and `mixed` (MixedImages) holds the files; to_device decodes them."""
+        self.buffer, self.items, self.mixed = pack_any([s[0] for s in samples])
         self.sizes = [(int(s[3][0]), int(s[3][1])) for s in samples]
         self.ids = [s[4] for s in samples]
         for i, (img, gt, bits, (h, w), _) in enumerate(s[:5] for s in samples):
@@ -133,11 +278,22 @@ class PackedValBatch:
     def pin_memory(self):
         """Called by DataLoader(pin_memory=True) in its pin thread: page-locks the images, the gts and the gt masks (and the
         annotation tables when there are any)."""
-        self.buffer, self.gt, self.gt_masks = self.buffer.pin_memory(), self.gt.pin_memory(), self.gt_masks.pin_memory()
+        if self.mixed is not None:
+            self.mixed.pin_memory()
+        else:
+            self.buffer = self.buffer.pin_memory()
+        self.gt, self.gt_masks = self.gt.pin_memory(), self.gt_masks.pin_memory()
         if self.ann_cls is not None:
             self.ann_cls, self.ann_box, self.ann_area, self.ann_crowd, self.ann_masks = (
                 t.pin_memory() for t in (self.ann_cls, self.ann_box, self.ann_area, self.ann_crowd, self.ann_masks))
         return self
+
+    def to_device(self, device):
+        """-> (CUDA uint8 buffer of the images in `items`' layout, device int32 status of the files decoded there or None); the
+        files are decoded by yb_jpeg_decode_batch, no host sync."""
+        if self.mixed is not None:
+            return self.mixed.to_device(device)
+        return self.buffer.to(device, non_blocking=self.buffer.is_pinned()), None
 
     def gt_to(self, device):
         """-> (gt [G,5], list of B packed gt masks [g_b, h_b, ceil(w_b/32)]) on `device`: views of one copy of each buffer."""

@@ -18,15 +18,14 @@ import os.path as osp
 
 import numpy as np
 
-from .augmentations import PackedTrainBatch, PackedValBatch, pack_images, train_aug_plan
+from .augmentations import EncodedImage, PackedTrainBatch, PackedValBatch, pack_any, read_image, train_aug_plan
 from .mask_utils import pack_masks_host
 
 
-def _imread(image_path, file_name):
-    import cv2
+def _imread(image_path, file_name, decode_gpu=False):
     img_path = osp.join(image_path, file_name)
     assert osp.exists(img_path), f'Image path does not exist: {img_path}'
-    return cv2.imread(img_path)
+    return read_image(img_path, decode_gpu)
 
 
 def train_collate(batch):
@@ -106,11 +105,16 @@ class COCOValDetection:
     With coco_eval=True each sample also carries every annotation of the image in file order, crowd ones included, for
     utils.cocoeval.CocoEvaluator: (class int32 [m] (continuous_id - 1), bbox float64 [m,4] (the annotation's x,y,w,h), area
     float64 [m], iscrowd int32 [m], masks bit-packed int32 [m,h,ceil(w/32)] (annToMask)).  The images visited, their order, len()
-    and the RuntimeError rule stay the same."""
+    and the RuntimeError rule stay the same.
 
-    def __init__(self, cfg, coco=None, coco_eval=False):
+    With decode_gpu=True the image is the file's bytes (utils.augmentations.EncodedImage, (h, w) from yb_jpeg_header) when
+    yb_jpeg_decode_batch decodes it, and the batch is decoded on the device (PackedValBatch.to_device); a file it refuses is read
+    by cv2.imread here, as without the flag."""
+
+    def __init__(self, cfg, coco=None, coco_eval=False, decode_gpu=False):
         self.cfg = cfg
         self.coco_eval = bool(coco_eval)
+        self.decode_gpu = bool(decode_gpu)
         self.image_path = cfg.val_imgs
         if coco is None:
             from pycocotools.coco import COCO
@@ -123,7 +127,7 @@ class COCOValDetection:
         return len(self.ids) if self.cfg.val_num == -1 else min(self.cfg.val_num, len(self.ids))
 
     def load_image(self, file_name):
-        return _imread(self.image_path, file_name)
+        return _imread(self.image_path, file_name, self.decode_gpu)
 
     def __getitem__(self, index):
         img_id = self.ids[index]
@@ -140,7 +144,7 @@ class COCOValDetection:
         assert masks.shape == (boxes.shape[0], height, width), 'Unmatched annotations.'
         boxes = boxes / np.array([width, height, width, height])
         gt = np.hstack((boxes, np.expand_dims(labels, axis=1))).astype(np.float32)
-        sample = (np.ascontiguousarray(img), gt, pack_masks_host(masks), (height, width), img_id)
+        sample = (img if isinstance(img, EncodedImage) else np.ascontiguousarray(img), gt, pack_masks_host(masks), (height, width), img_id)
         if not self.coco_eval:
             return sample
         ann = (np.array([self.continuous_id[a['category_id']] - 1 for a in anns], np.int32),
@@ -152,10 +156,12 @@ class COCOValDetection:
 class PackedDetectBatch:
     """A batch of images for yolact_minimal_b200.detect: `buffer` / `items` the raw uint8 BGR images back to back and their
     yb_val_aug_item table (pack_images), `names` their file names, `sizes` their (h, w).  With DataLoader(pin_memory=True) the
-    loader's pin thread page-locks the buffer."""
+    loader's pin thread page-locks the buffer.
+    With images given as JPEG files (EncodedImage) `buffer` is None until the device buffer is copied back, and `mixed`
+    (utils.augmentations.MixedImages) holds the files and the pixels of the others; to_device decodes them."""
 
     def __init__(self, images, names):
-        self.buffer, self.items = pack_images(images)
+        self.buffer, self.items, self.mixed = pack_any(images)
         self.names = list(names)
         self.sizes = [(int(h), int(w)) for _, h, w in self.items.tolist()]
 
@@ -163,8 +169,18 @@ class PackedDetectBatch:
         return len(self.items)
 
     def pin_memory(self):
-        self.buffer = self.buffer.pin_memory()
+        if self.mixed is not None:
+            self.mixed.pin_memory()
+        else:
+            self.buffer = self.buffer.pin_memory()
         return self
+
+    def to_device(self, device):
+        """-> (CUDA uint8 buffer of the images in `items`' layout, device int32 status of the files decoded there (entry k is image
+        mixed.encoded[k]) or None).  No host sync."""
+        if self.mixed is not None:
+            return self.mixed.to_device(device)
+        return self.buffer.to(device, non_blocking=self.buffer.is_pinned()), None
 
     def image(self, b):
         """Image b as a numpy view [h,w,3] of the (host) buffer."""
@@ -179,19 +195,20 @@ def detect_collate(batch):
 
 class DetectImages:
     """The reference's COCODetection(cfg, mode='detect') images (utils/coco.py:56-67): the sorted glob(cfg.image + '/*.jpg').
-    Returns (img_u8 [h,w,3] BGR, file name); val_aug runs on the device for a whole batch."""
+    Returns (img_u8 [h,w,3] BGR, file name); val_aug runs on the device for a whole batch.  With decode_gpu=True the image is the
+    file's bytes (EncodedImage) when yb_jpeg_decode_batch decodes it, and cv2.imread's pixels otherwise."""
 
-    def __init__(self, cfg):
+    def __init__(self, cfg, decode_gpu=False):
         self.image_path = glob.glob(cfg.image + '/*.jpg')
         self.image_path.sort()
+        self.decode_gpu = bool(decode_gpu)
 
     def __len__(self):
         return len(self.image_path)
 
     def __getitem__(self, index):
-        import cv2
         img_name = self.image_path[index]
-        img = cv2.imread(img_name)
+        img = read_image(img_name, self.decode_gpu)
         if img is None:
             raise RuntimeError(f'cannot read image {img_name}')
-        return np.ascontiguousarray(img), img_name.split(osp.sep)[-1]
+        return img if isinstance(img, EncodedImage) else np.ascontiguousarray(img), img_name.split(osp.sep)[-1]
