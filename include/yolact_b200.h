@@ -46,6 +46,12 @@ typedef enum {
 
 #define YB_VERSION 100
 
+/* Class counts (num_classes, background included) every entry point accepts: 2 .. YB_MAX_CLASSES.  The bound comes from the
+ * kernels that give each lane of a warp a fixed number of classes: C - 1 <= 128 foreground classes in the post-process, and
+ * at most 5 logits per lane in the head softmax.  yb_net_create and yb_train_create refuse a larger count with
+ * YB_ERR_UNSUPPORTED, yb_detect likewise, and yb_losses with YB_ERR_INVALID. */
+#define YB_MAX_CLASSES 129
+
 YB_API int yb_version(void);
 YB_API const char* yb_last_error(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches) */

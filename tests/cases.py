@@ -19,10 +19,10 @@ def nms_cases():
     return cases
 
 
-def build_nms_inputs(S, regime, seed, mut):
+def build_nms_inputs(S, regime, seed, mut, num_classes=81):
     anchors = pp.make_anchors(S)
     A = anchors.shape[0]
-    cls, box, coef = synth.head_outputs(seed, A, 81, regime)
+    cls, box, coef = synth.head_outputs(seed, A, num_classes, regime)
     if mut == 'dup_boxes':
         box[1::2] = box[0::2][:box[1::2].shape[0]]
         anchors = anchors.copy(); anchors[1::2] = anchors[0::2][:anchors[1::2].shape[0]]
@@ -31,7 +31,7 @@ def build_nms_inputs(S, regime, seed, mut):
     elif mut in ('few', 'none', 'one'):
         keep_n = {'few': 37, 'none': 0, 'one': 1}[mut]
         cls[:] = 0.0; cls[:, 0] = 1.0
-        src, _, _ = synth.head_outputs(seed + 1, A, 81, 'stress')
+        src, _, _ = synth.head_outputs(seed + 1, A, num_classes, 'stress')
         rows = (np.arange(keep_n) * 23 + 5) % A
         cls[rows] = src[rows]
     return anchors, cls, box, coef

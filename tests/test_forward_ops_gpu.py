@@ -36,8 +36,9 @@ errors (CUDA C Programming Guide, "Mathematical Functions", maximum ulp errors):
 Exact ops (max-pool, phase split, the stem's space-to-depth image, the head's box copy) must match exactly, halos and padding
 included.  16-bit results must stay below the fp16 saturation (65504) so the bound means something.  Structural checks: every
 haloed output except the attention output (whose halo is untouched by contract: the projection's epilogue zeroes its own) has
-an all-zero halo; the census of checked ops equals the program's; and at the two pipelined configurations the stepped outputs
-equal a normal yb_net_forward bit for bit (k_conv_tc / k_bneck_tc launch with programmatic dependent launch).
+an all-zero halo; the census of checked ops equals the program's; and at the pipelined configurations the stepped outputs
+equal a normal yb_net_forward bit for bit (k_conv_tc / k_bneck_tc launch with programmatic dependent launch).  The class-count
+configurations run the head at 21 (Pascal), 5 (the custom set) and the bounds 2 and 129.
 """
 import collections
 import ctypes
@@ -61,7 +62,7 @@ E24 = 2.0 ** -24
 U = {1: 2.0 ** -8, 2: 2.0 ** -11}
 ETA = {1: 2.0 ** -134, 2: 2.0 ** -25}
 TDT = {0: torch.float32, 1: torch.bfloat16, 2: torch.float16}
-NC, R, K = 81, 3, 32
+R, K = 3, 32
 KINDS = ['stem', 'pool', 'split', 'conv', 'upadd', 'up2x', 'headfin', 'patch_embed', 'ln', 'attn', 'merge_ln', 'bneck']
 DEPTH = {'res50': 50, 'res101': 101, 'swin_tiny': 0}
 BNECK_TRIPLES = {(64, 256, 64), (128, 512, 128), (256, 1024, 256), (64, 256, 128), (128, 512, 256)}
@@ -75,7 +76,16 @@ CONFIGS = {
     'swin-544-B2-fp16': dict(arch='swin_tiny', S=544, B=2, prec='fp16', max_batch=2),
     'res50-550-B3-fp16-stemwide': dict(arch='res50', S=550, B=3, prec='fp16', max_batch=3, stem_only=True,
                                        env={'YOLACT_B200_STEM_WIDE': '1'}),
+    # the class count (nc, background included; 81 when absent) sets the head conv's width, and with it the tile width
+    # conv_tc.cu's pick_bn gives it, and how many logits each lane of k_head_finalize holds
+    'res50-550-B2-bf16-nc21': dict(arch='res50', S=550, B=2, prec='bf16', max_batch=2, nc=21),
+    'res101-550-B2-fp16-nc5': dict(arch='res101', S=550, B=2, prec='fp16', max_batch=2, nc=5),
+    'res50-128-B2-fp16-nc2': dict(arch='res50', S=128, B=2, prec='fp16', max_batch=2, nc=2),
+    'res50-128-B2-bf16-nc129': dict(arch='res50', S=128, B=2, prec='bf16', max_batch=2, nc=129, pipelined=True),
 }
+# the head conv's row stride, R * (nc + 4 + K) rounded up to 16: 176 is one 176-wide tile with 5 padding columns, 496 is
+# 31 tiles of width 16
+HEAD_LD = {81: 352, 21: 176, 5: 128, 2: 128, 129: 496}
 
 
 def chunks(B, per_image):
@@ -179,6 +189,7 @@ class Stepped:
         c = CONFIGS[key]
         self.key, self.dev = key, dev
         self.arch, self.S, self.B, self.prec, self.mb = c['arch'], c['S'], c['B'], c['prec'], c['max_batch']
+        self.nc = c.get('nc', 81)
         torch.backends.cuda.matmul.allow_tf32 = False
         torch.backends.cudnn.allow_tf32 = False
         from yolact_minimal_b200 import _lib
@@ -187,14 +198,14 @@ class Stepped:
         old = {k: os.environ.get(k) for k in c.get('env', {})}
         os.environ.update(c.get('env', {}))
         try:
-            self.eng = Engine(DEPTH[self.arch], self.S, NC, R, K)
+            self.eng = Engine(DEPTH[self.arch], self.S, self.nc, R, K)
         finally:
             for k, v in old.items():
                 if v is None:
                     os.environ.pop(k, None)
                 else:
                     os.environ[k] = v
-        self.sd = ft.synth_state_dict(self.arch, seed=0)
+        self.sd = ft.synth_state_dict(self.arch, num_classes=self.nc, seed=0)
         self.eng.load_state(self.sd)
         with torch.cuda.device(dev):
             self.eng.finalize(self.mb, self.prec)
@@ -289,7 +300,7 @@ class Stepped:
         warm = torch.randn(self.mb, 3, S, S, device=dev, generator=gen) * 2.0
         gen.manual_seed(1234)
         self.img = torch.randn(B, 3, S, S, device=dev, generator=gen)
-        mk = lambda n: [torch.empty(n, A, NC, device=dev), torch.empty(n, A, 4, device=dev), torch.empty(n, A, K, device=dev),
+        mk = lambda n: [torch.empty(n, A, self.nc, device=dev), torch.empty(n, A, 4, device=dev), torch.empty(n, A, K, device=dev),
                         torch.empty(n, P, P, K, device=dev)]
         self.forward(warm, 0, self.n_ops, mk(self.mb))                     # stale data in every arena slot
         self.outs = [t.fill_(float('nan')) for t in mk(B)]
@@ -465,7 +476,8 @@ class Stepped:
             self.check_conv(f'{name} (proto out)', xf, taps, k, 1, b[:cout].double(), o['relu'], None, lambda b0, b1: out[b0:b1], n, dense=True)
         elif head:
             out = self.raw(o['out'])[0]
-            ncol = R * (NC + 4 + K)
+            ncol = R * (self.nc + 4 + K)
+            self.extents['head_ld'].add(out.shape[-1])
             self.check_conv(f'head conv {out.shape[1]}', xf, taps, k, 1, b[:cout].double(), o['relu'], None,
                             lambda b0, b1: out[b0:b1, ..., :ncol], n, dense=True)
         else:
@@ -519,7 +531,7 @@ class Stepped:
         self.forward(self.img, i, i + 1, self.outs)
         h = self.raw(o['in'])[0]
         H = h.shape[1]
-        n_a, a0 = H * H * R, o['anchor_offset']
+        n_a, a0, NC = H * H * R, o['anchor_offset'], self.nc
         lg = h.reshape(self.B, H * H, -1)[..., :R * (NC + 4 + K)]                # per pixel: conf R*NC | box R*4 | coef R*K
         conf = lg[..., :R * NC].reshape(self.B, n_a, NC).double()
         box = lg[..., R * NC:R * (NC + 4)].reshape(self.B, n_a, 4)
@@ -759,6 +771,7 @@ def test_every_op_is_checked(stepped):
     if r.arch != 'swin_tiny':
         assert r.extents['stem'] == {(16, r.S)}
     assert r.extents['headfin'] == {0, 1, 2, 3, 4}
+    assert r.extents['head_ld'] == {HEAD_LD[r.nc]}, r.extents['head_ld']
     if r.arch == 'swin_tiny':
         Hs = {550: (138, 69, 35, 18), 544: (136, 68, 34, 17)}[r.S]
         assert r.extents['attn'] == {(h, s) for h in Hs for s in (0, 3)}, r.extents['attn']
@@ -767,5 +780,5 @@ def test_every_op_is_checked(stepped):
 
 def test_stepped_equals_pipelined(stepped):
     if not CONFIGS[stepped.key].get('pipelined'):
-        pytest.skip('checked at the two pipelined configurations')
+        pytest.skip('checked at the pipelined configurations')
     assert stepped.pipelined_equal, 'the op-by-op run differs from yb_net_forward'

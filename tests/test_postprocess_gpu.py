@@ -15,9 +15,12 @@ from oracle import synth, postprocess_np as pp
 pytestmark = pytest.mark.gpu
 
 
-def _cfg(traditional=False, S=544, **kw):
+def _cfg(traditional=False, S=544, classes='res101_coco', **kw):
+    """classes: a config name, or a class count (background included) for res101_coco's settings at that count."""
     from yolact_minimal_b200.config import make_config
-    cfg = make_config('res101_coco', S, traditional_nms=traditional)
+    cfg = make_config('res101_coco' if isinstance(classes, int) else classes, S, traditional_nms=traditional)
+    if isinstance(classes, int):
+        cfg.num_classes = classes
     for k, v in kw.items():
         setattr(cfg, k, v)
     return cfg
@@ -172,6 +175,41 @@ def test_sampled_cuts_cannot_change_the_result(cuda):
     r = _run(cuda, cls, box, coef, anchors, _cfg(S=S))
     for b in range(4):
         _check_image(r, b, pp.nms(cls[b], box[b], anchors), coef[b])
+
+
+# Pascal's 21 and the custom set's 5 classes, and the bounds: 2 classes launch one block per image in the per-class stages, 129
+# (C1 = 128) fill all four class slots of every lane of k_sample_cuts and every [128] shared array of the phase-1 kernels
+CLASS_COUNTS = (2, 5, 21, 129)
+
+
+def largest_max_det(C):
+    """The largest max_det <= 256 whose final top-k keys (2 C1 max_det words after C1 counts) fit its 200 KiB."""
+    C1 = C - 1
+    return min(256, (200 * 1024 - 4 * ((C1 + 3) & ~3)) // (8 * C1))
+
+
+@pytest.mark.parametrize('C', CLASS_COUNTS)
+@pytest.mark.parametrize('S', [550, 128])
+def test_class_counts_vs_oracle(cuda, S, C):
+    """Fast-NMS and traditional NMS at C classes, bit for bit against the oracle: at S = 550 (A = 19 248 > 2048, so the per-class
+    lists are filled from k_sample_cuts' sampled cuts) and S = 128 (A = 1023, no sampling).  One batch holds a stress image, a
+    realistic one and a stress image with scores quantised to 1/16, whose tied groups straddle every max_det cut."""
+    anchors = pp.make_anchors(S)
+    assert (anchors.shape[0] > 2048) == (S == 550)
+    items = [build_nms_inputs(S, reg, seed, None, C) for reg, seed in (('stress', 31), ('realistic', 32), ('stress', 33))]
+    cls = np.stack([i[1] for i in items]); box = np.stack([i[2] for i in items]); coef = np.stack([i[3] for i in items])
+    cls[2] = (np.round(cls[2] * 16) / 16).astype(np.float32)
+    md_max = largest_max_det(C)
+    assert (md_max < 256) == (C == 129)
+    trad = [pp.nms(cls[b], box[b], anchors, max_det=10 ** 9, traditional=True, img_size=S) for b in range(3)]
+    assert trad[0] is not None and len(trad[0][0]) > 1
+    for top_k, max_det in ((200, 100), (7, 5), (1, 1), (256, md_max)):
+        r = _run(cuda, cls, box, coef, anchors, _cfg(S=S, classes=C, top_k=top_k, max_detections=max_det))
+        for b in range(3):
+            _check_image(r, b, pp.nms(cls[b], box[b], anchors, top_k=top_k, max_det=max_det), coef[b])
+        r = _run(cuda, cls, box, coef, anchors, _cfg(True, S=S, classes=C, max_detections=max_det))
+        for b in range(3):
+            _check_image(r, b, None if trad[b] is None else tuple(a[:max_det] for a in trad[b]), coef[b])
 
 
 def test_hard_nms_vs_oracle_and_golden(cuda):

@@ -162,12 +162,12 @@ def test_tied_overlapping_boxes(cuda):
         _check_image(r, 0, _cut(o, md), coef)
 
 
-def _raw_detect(cuda, cls, box, coef, anchors, S, fill):
+def _raw_detect(cuda, cls, box, coef, anchors, S, fill, max_det=100, traditional=1):
     """yb_detect with output and workspace buffers the caller owns, pre-filled with `fill` bytes."""
     from yolact_minimal_b200 import _lib
     B, A, C = cls.shape
-    K, D = coef.shape[-1], 100
-    p = _lib.DetectParams(0.05, 0.5, 200, D, C, K, 1, float(S), 0)
+    K, D = coef.shape[-1], max_det
+    p = _lib.DetectParams(0.05, 0.5, 200, D, C, K, traditional, float(S), 0)
     L = _lib.lib()
     nbytes = int(L.yb_detect_workspace_bytes(B, A, ctypes.byref(p)))
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(cuda)

@@ -45,12 +45,18 @@ DT = {'bf16': torch.bfloat16, 'fp16': torch.float16}
 # ambiguous only inside this window around it, and there the engine's and the checker's dY may differ by one ulp
 LOSS_GRAD_EPS = 2.0 ** -16
 
-# (arch, S, B, precision, big-mean stem channel, which bottleneck blocks are checked (None = all))
+# (arch, S, B, precision, big-mean stem channel, which bottleneck blocks are checked (None = all)[, config name[, class count]])
+# The config name defaults to arch + '_coco'; the class count (background included) to the config's.  The class count sizes the
+# head conv (3 (NC + 36) columns), the seg conv (NC - 1: Cout = 1 at two classes) and k_head_train / k_head_grad's row addressing.
 CONFIGS = {
     'res50-550-B2-bf16': ('res50', 550, 2, 'bf16', False, None),
     'res101-550-B2-bf16': ('res101', 550, 2, 'bf16', False, {'0.0', '1.0', '2.0', '2.1', '2.22', '3.0'}),
     'res50-550-B3-fp16': ('res50', 550, 3, 'fp16', True, None),
     'res50-128-B2-fp16': ('res50', 128, 2, 'fp16', False, None),
+    'pascal-550-B2-bf16': ('res50', 550, 2, 'bf16', False, None, 'res50_pascal'),
+    'custom-res101-550-B2-fp16': ('res101', 550, 2, 'fp16', False, {'0.0', '1.0', '2.0', '2.1', '2.22', '3.0'}, 'res101_custom'),
+    'nc2-128-B2-fp16': ('res50', 128, 2, 'fp16', False, None, None, 2),
+    'nc129-128-B2-bf16': ('res50', 128, 2, 'bf16', False, None, None, 129),
 }
 MEAN_SHIFT = 30.0            # added to the image; channel 0 of the stem sees no zero padding, so its |mean| / std is ~ 3 * shift
 
@@ -119,13 +125,13 @@ def graph(depth, R, NC, K):
 # ------------------------------------------------------------------------------------------------
 class Run:
     def __init__(self, key, dev):
-        arch, S, B, prec, shift, blocks = CONFIGS[key]
+        arch, S, B, prec, shift, blocks, config, nc = (CONFIGS[key] + (None, None))[:8]
         self.key, self.arch, self.S, self.B, self.prec, self.blocks, self.dev = key, arch, S, B, prec, blocks, dev
         self.u, self.dt = U[prec], DT[prec]
         torch.backends.cudnn.allow_tf32 = False
         torch.backends.cuda.matmul.allow_tf32 = False
         from oracle import synth
-        net = tc.make_train_net(arch, S, B, dev)
+        net = tc.make_train_net(arch, S, B, dev, config, nc)
         net.cfg.train_precision = prec
         img = torch.from_numpy(synth.image_batch(11, B, S)).to(dev)
         if shift:
@@ -135,7 +141,7 @@ class Run:
                 keep[3:5, 3:5] = 1
                 w[0] = w[0].abs() * keep
             img = img + MEAN_SHIFT
-        tg, mk = synth.train_targets(5, B, S)
+        tg, mk = synth.train_targets(5, B, S, num_classes=net.cfg.num_classes - 1)
         self.tg, self.mk = tg, mk
         tgt = [torch.from_numpy(t).to(dev) for t in tg]
         mks = [torch.from_numpy(m).to(dev) for m in mk]

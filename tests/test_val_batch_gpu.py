@@ -3,7 +3,8 @@
   * after_nms_batched == yb_mask_assemble(mask_f32 = 2) per image on the first count[b] detections, masks and boxes; rows past
     count[b] are zero boxes and write no mask word (sentinels around every image's range and at the buffer's tail stay);
   * host-packed gt masks == yb_pack_mask_bits;
-  * evaluate() == the reference's per-image loop (tests/val_loop.py), tables compared with ==, at res101 550 fp16;
+  * evaluate() == the reference's per-image loop (tests/val_loop.py), tables compared with ==, at res101 550 fp16, and at
+    res50_pascal (21 classes, identity category ids);
   * library launches per batch do not depend on B or the detections, and the per-batch body never synchronises."""
 
 import numpy as np
@@ -173,12 +174,13 @@ EVAL_SIZES = [(480, 640), (640, 480), (427, 640), (550, 550), (300, 200), (64, 9
 
 def _eval_set(tmp_path, net, cfg, n=45):
     """n synthetic PNG images on disk; gts from a first detection pass (shifted boxes of some detections, an unrelated box, one
-    crowd annotation), as in test_eval_gpu.py's end-to-end case."""
+    crowd annotation), as in test_eval_gpu.py's end-to-end case.  Category ids are the config's: COCO's for the COCO configs, the
+    identity map of cfg.continuous_id otherwise."""
     import cv2
-    from yolact_minimal_b200.config import COCO_LABEL_MAP
     from yolact_minimal_b200.utils.augmentations import val_aug
     from yolact_minimal_b200.utils.output_utils import after_nms, nms
-    coco_id = {label - 1: cid for cid, label in COCO_LABEL_MAP.items()}
+    cat_id = {label - 1: cid for cid, label in cfg.continuous_id.items()}
+    nfg = cfg.num_classes - 1
     rng = np.random.RandomState(9)
     images = {}
     dev = next(net.parameters()).device
@@ -200,44 +202,74 @@ def _eval_set(tmp_path, net, cfg, n=45):
             ids = ids_p.cpu().numpy()
             for i in range(0, len(ids), 3):
                 x1, y1, x2, y2 = np.clip(bx[i] + [2, -1, 3, 1], 0, [w, h, w, h])
-                anns.append(dict(bbox=[x1, y1, x2 - x1, y2 - y1], category_id=coco_id[int(ids[i])], iscrowd=0))
-        anns.append(dict(bbox=[5.0, 5.0, 35.0, 25.0], category_id=coco_id[(7 * k) % 80], iscrowd=0))
-        anns.append(dict(bbox=[1.0, 2.0, 20.0, 20.0], category_id=coco_id[k % 80], iscrowd=1))
+                anns.append(dict(bbox=[x1, y1, x2 - x1, y2 - y1], category_id=cat_id[int(ids[i])], iscrowd=0))
+        anns.append(dict(bbox=[5.0, 5.0, 35.0, 25.0], category_id=cat_id[(7 * k) % nfg], iscrowd=0))
+        anns.append(dict(bbox=[1.0, 2.0, 20.0, 20.0], category_id=cat_id[k % nfg], iscrowd=1))
         for a in anns:
             a['_hw'] = (h, w)
         images[1000 + k] = (name, h, w, anns)
     return _StubCOCO(images)
 
 
-@pytest.fixture(scope='module')
-def res101(cuda):
+def _synthetic_net(dev, config, arch):
+    """An eval-mode Yolact of `config` at 550 fp16 with synthetic weights of its class count."""
+    import time
     from oracle import forward_torch as ft
     from yolact_minimal_b200.config import make_config
     from yolact_minimal_b200.modules.yolact import Yolact
-    cfg = make_config('res101_coco', 550, mode='val')
+    t0 = time.time()
+    torch.cuda.reset_peak_memory_stats()
+    cfg = make_config(config, 550, mode='val')
     cfg.precision, cfg.max_batch = 'fp16', 64
     net = Yolact(cfg)
-    net.load_state_dict(ft.synth_state_dict('res101', seed=0), strict=True)
-    return net.to(cuda).eval(), cfg
+    net.load_state_dict(ft.synth_state_dict(arch, num_classes=cfg.num_classes, seed=0), strict=True)
+    net = net.to(dev).eval()
+    print(f'\n{config}: net built in {time.time() - t0:.1f} s, peak memory {torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB')
+    return net, cfg
 
 
-@pytest.mark.parametrize('traditional', [False, True])
-def test_evaluate_equals_per_image_loop(res101, tmp_path, traditional):
+@pytest.fixture(scope='module')
+def res101(cuda):
+    return _synthetic_net(cuda, 'res101_coco', 'res101')
+
+
+@pytest.fixture(scope='module')
+def pascal(cuda):
+    """res50_pascal: 21 classes, category ids 1..20 through the identity continuous_id."""
+    return _synthetic_net(cuda, 'res50_pascal', 'res50')
+
+
+def _evaluate_equals_per_image_loop(net, cfg, tmp_path, traditional, val_bss):
+    import time
     from val_loop import per_image_evaluate
     from yolact_minimal_b200.eval import evaluate
     from yolact_minimal_b200.utils.coco import COCOValDetection
-    net, cfg = res101
+    t0 = time.time()
     cfg.traditional_nms = traditional
     cfg.val_imgs = str(tmp_path)
     coco = _eval_set(tmp_path, net, cfg)
     ds = COCOValDetection(cfg, coco=coco)
     want = per_image_evaluate(net, cfg, (ds[i] for i in range(len(ds))))
     assert want[1][1] > 0 and want[2][1] > 0                                 # the case has matches in both types
-    for val_bs in (1, 8, 64):
+    for val_bs in val_bss:
         for workers in (0, 2):
             cfg.val_bs = val_bs
             got = evaluate(net, cfg, dataset=ds, num_workers=workers)
             assert got == want, (val_bs, workers, got[1:], want[1:])
+    print(f'{type(cfg).__name__} traditional={traditional}: {time.time() - t0:.1f} s, peak memory '
+          f'{torch.cuda.max_memory_allocated() / 2 ** 30:.1f} GiB')
+
+
+@pytest.mark.parametrize('traditional', [False, True])
+def test_evaluate_equals_per_image_loop(res101, tmp_path, traditional):
+    _evaluate_equals_per_image_loop(*res101, tmp_path, traditional, (1, 8, 64))
+
+
+@pytest.mark.parametrize('traditional', [False, True])
+def test_pascal_evaluate_equals_per_image_loop(pascal, tmp_path, traditional):
+    net, cfg = pascal
+    assert cfg.num_classes == 21 and cfg.continuous_id == {i: i for i in range(1, 21)}
+    _evaluate_equals_per_image_loop(net, cfg, tmp_path, traditional, (1, 8))
 
 
 def _batch_body(net, cfg, packed, ev, dev):

@@ -92,12 +92,16 @@ def torch_losses_and_grads(cfg, anchors, tg, mk, class_p, box_p, coef_p, proto_p
                                             d_seg=seg.grad.numpy())
 
 
-def make_train_net(arch, S, B, dev):
+def make_train_net(arch, S, B, dev, config=None, num_classes=None):
+    """A training-mode Yolact with synthetic weights.  config: a config name (default arch + '_coco'); num_classes (background
+    included) overrides the config's class count, for the counts no config has."""
     from yolact_minimal_b200.config import make_config
     from yolact_minimal_b200.modules.yolact import Yolact
-    cfg = make_config(arch + '_coco', S, mode='train', train_bs=B)
+    cfg = make_config(config or arch + '_coco', S, mode='train', train_bs=B)
+    if num_classes is not None:
+        cfg.num_classes = num_classes
     net = Yolact(cfg)
-    net.load_state_dict(ft.synth_state_dict(arch, seed=0, train=True), strict=True)
+    net.load_state_dict(ft.synth_state_dict(arch, num_classes=cfg.num_classes, seed=0, train=True), strict=True)
     return net.to(dev).train()
 
 
@@ -144,7 +148,7 @@ def engine_vs_checker(arch, S, B, dev, precision='bf16', img_seed=11, tgt_seed=5
             try:
                 if name.startswith('out.'):
                     v = eng.read_output(name[4:])
-                    cache[name] = v[..., :80].permute(0, 3, 1, 2).contiguous() if name == 'out.seg' else v      # engine: NHWC; checker: NCHW
+                    cache[name] = v[..., :net.cfg.num_classes - 1].permute(0, 3, 1, 2).contiguous() if name == 'out.seg' else v   # engine: NHWC; checker: NCHW
                 else:
                     cache[name] = eng.read(name)
             except Exception:

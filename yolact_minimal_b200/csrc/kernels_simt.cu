@@ -544,6 +544,7 @@ int launch_upsample2x_ac(const void* in, void* out, int dt, int B, int C, int Hi
 // contiguous runs of R*NC, R*4 and R*K floats in the outputs.  (The first version gave each warp one (pixel, anchor) item and read
 // its 81 + 4 + 32 values with partially filled, misaligned loads: 2.9 TB/s; profiles/r2_glue_kernels.txt.)
 constexpr int kHeadWarps = 8;
+constexpr int kHeadLogitsPerLane = (YB_MAX_CLASSES + 31) / 32;          // class c is lane c % 32's logit c / 32
 
 __global__ void __launch_bounds__(kHeadWarps * 32) k_head_finalize(const float* __restrict__ head, int ld, int HW, int R, int NC, int K,
                                                                    int anchor_offset, int A_total, float* __restrict__ cls,
@@ -560,21 +561,24 @@ __global__ void __launch_bounds__(kHeadWarps * 32) k_head_finalize(const float* 
   __syncwarp();
   const size_t arow = (size_t)b * A_total + anchor_offset + (size_t)pix * R;   // first of the pixel's R anchors
   for (int a = 0; a < R; ++a) {
-    float lg[4];
+    float lg[kHeadLogitsPerLane], mx = -INFINITY;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) { const int c = lane + 32 * i; lg[i] = c < NC ? sr[a * NC + c] : -INFINITY; }
-    float mx = fmaxf(fmaxf(lg[0], lg[1]), fmaxf(lg[2], lg[3]));
+    for (int i = 0; i < kHeadLogitsPerLane; ++i) {
+      const int c = lane + 32 * i;
+      lg[i] = c < NC ? sr[a * NC + c] : -INFINITY;
+      mx = fmaxf(mx, lg[i]);
+    }
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, off));
-    float ex[4], sum = 0.f;
+    float ex[kHeadLogitsPerLane], sum = 0.f;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) { ex[i] = (lane + 32 * i) < NC ? __expf(lg[i] - mx) : 0.f; sum += ex[i]; }
+    for (int i = 0; i < kHeadLogitsPerLane; ++i) { ex[i] = (lane + 32 * i) < NC ? __expf(lg[i] - mx) : 0.f; sum += ex[i]; }
 #pragma unroll
     for (int off = 16; off > 0; off >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, off);
     const float inv = 1.f / sum;
     __syncwarp();                                                      // every lane has read this anchor's logits
 #pragma unroll
-    for (int i = 0; i < 4; ++i) { const int c = lane + 32 * i; if (c < NC) sr[a * NC + c] = ex[i] * inv; }
+    for (int i = 0; i < kHeadLogitsPerLane; ++i) { const int c = lane + 32 * i; if (c < NC) sr[a * NC + c] = ex[i] * inv; }
   }
   __syncwarp();
   float* co = cls + arow * NC;
@@ -586,7 +590,8 @@ __global__ void __launch_bounds__(kHeadWarps * 32) k_head_finalize(const float* 
 
 int launch_head_finalize(const float* head, int ld, int B, int HW, int R, int NC, int K, int anchor_offset, int A_total,
                          float* cls, float* box, float* coef, cudaStream_t s) {
-  YB_REQUIRE(NC <= 128 && K <= 64 && R * 4 <= 32, YB_ERR_UNSUPPORTED, "head_finalize: num_classes=%d > 128, coef_dim=%d > 64 or %d ratios", NC, K, R);
+  YB_REQUIRE(NC <= YB_MAX_CLASSES && K <= 64 && R * 4 <= 32, YB_ERR_UNSUPPORTED, "head_finalize: num_classes=%d > %d, coef_dim=%d > 64 or %d ratios",
+             NC, YB_MAX_CLASSES, K, R);
   YB_REQUIRE(ld % 4 == 0 && R * (NC + 4 + K) <= ld && (size_t)kHeadWarps * ld * 4 <= 48 * 1024, YB_ERR_UNSUPPORTED, "head_finalize: row stride %d", ld);
   dim3 grid(ceil_div(HW, kHeadWarps), B);
   k_head_finalize<<<grid, kHeadWarps * 32, (size_t)kHeadWarps * ld * 4, s>>>(head, ld, HW, R, NC, K, anchor_offset, A_total, cls, box, coef);

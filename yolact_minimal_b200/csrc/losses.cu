@@ -532,7 +532,7 @@ int losses_impl(const yb_loss_params* p, const float* cls, const float* box, con
                 float* d_seg, int32_t* dbg_labels, int32_t* dbg_matched_idx, float* dbg_offsets, uint8_t* dbg_neg, void* workspace, size_t workspace_bytes,
                 void* stream) {
   YB_REQUIRE(p && cls && box && coef && proto && seg && anchors && gt && gt_offset && gt_masks && losses && workspace, YB_ERR_INVALID, "yb_losses: NULL argument");
-  YB_REQUIRE(p->batch >= 1 && p->num_anchors >= 1 && p->num_classes >= 2 && p->num_classes <= 129, YB_ERR_INVALID, "yb_losses: batch=%d anchors=%d classes=%d",
+  YB_REQUIRE(p->batch >= 1 && p->num_anchors >= 1 && p->num_classes >= 2 && p->num_classes <= YB_MAX_CLASSES, YB_ERR_INVALID, "yb_losses: batch=%d anchors=%d classes=%d",
              p->batch, p->num_anchors, p->num_classes);
   YB_REQUIRE(p->coef_dim >= 1 && p->coef_dim <= 32, YB_ERR_UNSUPPORTED, "yb_losses: coef_dim=%d (<= 32)", p->coef_dim);
   YB_REQUIRE(p->masks_to_train >= 1 && p->masks_to_train <= kMaxSel, YB_ERR_UNSUPPORTED, "yb_losses: masks_to_train=%d (<= %d)", p->masks_to_train, kMaxSel);

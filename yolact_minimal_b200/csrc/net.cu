@@ -557,6 +557,7 @@ extern "C" int yb_net_create(const yb_net_config* cfg, yb_net** out) {
   YB_REQUIRE(cfg->depth == 50 || cfg->depth == 101 || cfg->depth == 0, YB_ERR_UNSUPPORTED, "yb_net_create: depth=%d (50, 101, or 0 = Swin-T)", cfg->depth);
   YB_REQUIRE(cfg->img_size >= 64 && cfg->img_size <= 4096, YB_ERR_INVALID, "yb_net_create: img_size=%d", cfg->img_size);
   YB_REQUIRE(cfg->num_classes >= 2 && cfg->num_ratios >= 1 && cfg->num_ratios <= 3, YB_ERR_INVALID, "yb_net_create: num_classes=%d num_ratios=%d", cfg->num_classes, cfg->num_ratios);
+  YB_REQUIRE(cfg->num_classes <= YB_MAX_CLASSES, YB_ERR_UNSUPPORTED, "yb_net_create: num_classes=%d > %d", cfg->num_classes, YB_MAX_CLASSES);
   YB_REQUIRE(cfg->coef_dim > 0 && cfg->coef_dim % 4 == 0 && cfg->coef_dim <= 64, YB_ERR_UNSUPPORTED, "yb_net_create: coef_dim=%d", cfg->coef_dim);
   yb_net* net = new yb_net();
   net->cfg = *cfg;

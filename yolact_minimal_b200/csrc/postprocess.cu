@@ -917,6 +917,12 @@ k_hard_nms(const float* __restrict__ dets, int n, float thresh, uint8_t* keep /*
 // ================================================================================================
 using namespace yb;
 
+// k_final_topk's dynamic shared memory: [C1] counts, then [C1 * max_det] keys and as many tie keys
+static size_t final_topk_smem(int C1, int max_det) {
+  return (size_t)((C1 + 3) & ~3) * sizeof(int) + (size_t)2 * C1 * max_det * sizeof(uint32_t);
+}
+
+// every refusal happens here or before the first launch of yb_detect: a refused call writes nothing
 static int check_params(const yb_detect_params* p, int batch, int A) {
   YB_REQUIRE(p != nullptr, YB_ERR_INVALID, "yb_detect: params is NULL");
   YB_REQUIRE(batch > 0 && A > 0, YB_ERR_INVALID, "yb_detect: batch=%d num_anchors=%d", batch, A);
@@ -925,7 +931,9 @@ static int check_params(const yb_detect_params* p, int batch, int A) {
   YB_REQUIRE(p->max_det >= 1 && p->max_det <= kSortCap, YB_ERR_UNSUPPORTED, "yb_detect: max_det=%d outside [1,%d]", p->max_det, kSortCap);
   YB_REQUIRE(p->coef_dim >= 0, YB_ERR_INVALID, "yb_detect: coef_dim=%d", p->coef_dim);
   YB_REQUIRE((double)(p->num_classes - 1) * A < 4294967296.0, YB_ERR_UNSUPPORTED, "yb_detect: (C-1)*A overflows 32 bits");
-  YB_REQUIRE(p->num_classes <= 129, YB_ERR_UNSUPPORTED, "yb_detect: num_classes=%d > 129", p->num_classes);
+  YB_REQUIRE(p->num_classes <= YB_MAX_CLASSES, YB_ERR_UNSUPPORTED, "yb_detect: num_classes=%d > %d", p->num_classes, YB_MAX_CLASSES);
+  YB_REQUIRE(final_topk_smem(p->num_classes - 1, p->max_det) <= 200 * 1024, YB_ERR_UNSUPPORTED,
+             "yb_detect: (C-1)*max_det = %d too large for the final top-k stage", (p->num_classes - 1) * p->max_det);
   return YB_OK;
 }
 
@@ -989,8 +997,7 @@ extern "C" int yb_detect(const float* cls, const float* box, const float* coef, 
     YB_CHECK_LAUNCH();
   }
   {
-    const size_t smem = (size_t)((C1 + 3) & ~3) * sizeof(int) + (size_t)2 * C1 * p->max_det * sizeof(uint32_t);
-    YB_REQUIRE(smem <= 200 * 1024, YB_ERR_UNSUPPORTED, "yb_detect: (C-1)*max_det = %d too large for the final top-k stage", C1 * p->max_det);
+    const size_t smem = final_topk_smem(C1, p->max_det);
     YB_CHECK_CUDA(cudaFuncSetAttribute(k_final_topk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     k_final_topk<<<B, kThreads, smem, stream>>>(coef, A, C1, p->max_det, p->coef_dim, p->traditional, p->img_size, ws,
                                                  out_count, out_class, out_anchor, out_score, out_box, out_coef);

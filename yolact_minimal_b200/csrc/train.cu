@@ -1013,7 +1013,7 @@ extern "C" int yb_train_create(const yb_net_config* cfg, int batch, int precisio
              "yb_train_create: depth=%d (the training engine covers ResNet-50 / 101 and Swin-T, depth 0)", cfg->depth);
   YB_REQUIRE(batch >= 1 && batch <= 256, YB_ERR_INVALID, "yb_train_create: batch=%d", batch);
   YB_REQUIRE(precision == YB_PREC_BF16 || precision == YB_PREC_FP16, YB_ERR_UNSUPPORTED, "yb_train_create: precision=%d (bf16 or fp16 operands)", precision);
-  YB_REQUIRE(cfg->coef_dim == 32 && cfg->num_ratios >= 1 && cfg->num_ratios <= 3 && cfg->num_classes >= 2 && cfg->num_classes <= 129, YB_ERR_UNSUPPORTED,
+  YB_REQUIRE(cfg->coef_dim == 32 && cfg->num_ratios >= 1 && cfg->num_ratios <= 3 && cfg->num_classes >= 2 && cfg->num_classes <= YB_MAX_CLASSES, YB_ERR_UNSUPPORTED,
              "yb_train_create: coef_dim=%d num_ratios=%d num_classes=%d", cfg->coef_dim, cfg->num_ratios, cfg->num_classes);
   int cc_major = 0;
   YB_PROPAGATE(yb_device_info(nullptr, &cc_major, nullptr));
