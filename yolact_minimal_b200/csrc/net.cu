@@ -2,6 +2,7 @@
 // and weight packing, the flat layer program (modules/resnet.py:86-98 + modules/yolact.py:73-89,
 // :49-53, :26-31, :141-164 restated as a list of GEMM-shaped convs on haloed NHWC tensors),
 // a liveness-based activation arena, and the yb_net_* C ABI.
+#include "arch.cuh"
 #include "layers.cuh"
 
 #include <math.h>
@@ -149,10 +150,9 @@ int new_conv(yb_net* net, const std::string& wname, const std::string& bname, co
 int add_conv(yb_net* net, int in, int conv, int stride, int relu, int res = -1, int out_mode = 0, int ext = EXT_NONE, int out_act = -1) {
   const ConvW& c = net->convs[conv];
   const int Hin = net->acts[in].H;
-  int Hout = Hin;
+  const int Hout = out_size(Hin, stride);
   int src = in;
   if (stride == 2) {
-    Hout = (Hin - 1) / 2 + 1;
     const int planes = c.k == 3 ? 4 : 1;
     src = new_act(net, c.Cin, Hout, planes);
     Op sp; sp.kind = OP_SPLIT; sp.in = in; sp.out = src;
@@ -168,22 +168,19 @@ int add_conv(yb_net* net, int in, int conv, int stride, int relu, int res = -1, 
 
 void build_program(yb_net* net) {
   const yb_net_config& cfg = net->cfg;
-  const int S = cfg.img_size;
-  net->H1 = (S - 1) / 2 + 1;
-  net->H2 = (net->H1 - 1) / 2 + 1;
+  const StemSizes ss = stem_sizes(cfg.img_size);
+  net->H1 = ss.H1; net->H2 = ss.H2;
   int couts[4] = {-1, -1, -1, -1};
   int fin[3] = {512, 1024, 2048};
   if (cfg.depth == 0) {
     // ---------------- Swin-T backbone (modules/swin_transformer.py:436-518) ----------------
-    const int depths[4] = {2, 2, 6, 2}, heads[4] = {3, 6, 12, 24};
     fin[0] = 192; fin[1] = 384; fin[2] = 768;
-    int Hg = (S + 3) / 4;
-    net->H1 = Hg;
+    net->H1 = ss.Hg;
     net->add_param("backbone.patch_embed.proj.weight", 96 * 3 * 4 * 4);
     net->add_param("backbone.patch_embed.proj.bias", 96);
     net->add_param("backbone.patch_embed.norm.weight", 96);
     net->add_param("backbone.patch_embed.norm.bias", 96);
-    int x = new_act(net, 96, Hg);
+    int x = new_act(net, 96, ss.Hg);
     { Op o; o.kind = OP_PATCH_EMBED; o.out = x; net->ops.push_back(o); }
     auto add_ln = [&](int in, const std::string& name, int C) {
       net->add_param(name + ".weight", C); net->add_param(name + ".bias", C);
@@ -194,16 +191,16 @@ void build_program(yb_net* net) {
     };
     for (int s = 0; s < 4; ++s) {
       const int C = 96 << s;
-      for (int b = 0; b < depths[s]; ++b) {
+      for (int b = 0; b < kSwinDepths[s]; ++b) {
         const std::string p = "backbone.layers." + std::to_string(s) + ".blocks." + std::to_string(b);
         const int t1 = add_ln(x, p + ".norm1", C);
-        net->add_param(p + ".attn.relative_position_bias_table", 169 * heads[s]);
+        net->add_param(p + ".attn.relative_position_bias_table", 169 * kSwinHeads[s]);
         const int cq = new_conv(net, p + ".attn.qkv.weight", p + ".attn.qkv.bias", "", C, 3 * C, 1);
         const int cp = new_conv(net, p + ".attn.proj.weight", p + ".attn.proj.bias", "", C, C, 1);
         const int qkv = add_conv(net, t1, cq, 1, 0);
         const int att = new_act(net, C, net->acts[x].H);
         { Op o; o.kind = OP_ATTN; o.in = qkv; o.out = att; o.p0 = p + ".attn.qkv.bias"; o.p1 = p + ".attn.relative_position_bias_table";
-          o.heads = heads[s]; o.shift = (b % 2) ? 3 : 0; net->ops.push_back(o); }
+          o.heads = kSwinHeads[s]; o.shift = (b % 2) ? 3 : 0; net->ops.push_back(o); }
         x = add_conv(net, att, cp, 1, 0, x);                         // x + proj(attn)
         const int t2 = add_ln(x, p + ".norm2", C);
         const int c1 = new_conv(net, p + ".mlp.fc1.weight", p + ".mlp.fc1.bias", "", C, 4 * C, 1);
@@ -241,8 +238,7 @@ void build_program(yb_net* net) {
   int x = new_act(net, 64, net->H2);
   { Op o; o.kind = OP_POOL; o.in = stem; o.out = x; net->ops.push_back(o); }
 
-  const int nblk50[4] = {3, 4, 6, 3}, nblk101[4] = {3, 4, 23, 3};
-  const int* nblk = cfg.depth == 50 ? nblk50 : nblk101;
+  const int* nblk = resnet_blocks(cfg.depth);
   int inpl = 64;
   for (int s = 0; s < 4; ++s) {
     const int planes = 64 << s;
@@ -308,46 +304,20 @@ void build_program(yb_net* net) {
   add_conv(net, t, new_conv(net, "proto_net.proto2.2.weight", "proto_net.proto2.2.bias", "", 256, cfg.coef_dim, 1), 1, 1, -1, 1, EXT_PROTO);
 
   // prediction heads, shared weights over 5 levels (modules/yolact.py:12-31,:149-157)
-  const int R = cfg.num_ratios, NC = cfg.num_classes, K = cfg.coef_dim;
   const int upf = new_conv(net, "prediction_layers.upfeature.0.weight", "prediction_layers.upfeature.0.bias", "", 256, 256, 3);
-  ConvW hc; hc.Cin = 256; hc.Cin_pad = 256; hc.k = 3; hc.Cout = R * (NC + 4 + K); hc.Cout_pad = (hc.Cout + 15) / 16 * 16;
-  hc.cat = {"prediction_layers.conf_layer", "prediction_layers.bbox_layer", "prediction_layers.coef_layer.0"};
-  net->add_param("prediction_layers.bbox_layer.weight", (int64_t)R * 4 * 256 * 9);
-  net->add_param("prediction_layers.bbox_layer.bias", R * 4);
-  net->add_param("prediction_layers.conf_layer.weight", (int64_t)R * NC * 256 * 9);
-  net->add_param("prediction_layers.conf_layer.bias", R * NC);
-  net->add_param("prediction_layers.coef_layer.0.weight", (int64_t)R * K * 256 * 9);
-  net->add_param("prediction_layers.coef_layer.0.bias", R * K);
+  const HeadLayout hl = head_layout(cfg);
+  ConvW hc; hc.Cin = 256; hc.Cin_pad = 256; hc.k = 3; hc.Cout = hl.Cout; hc.Cout_pad = hl.Cout_pad; hc.cat = hl.cat;
+  for (const auto& p : hl.params) net->add_param(p.first, p.second);
   net->convs.push_back(hc);
   const int head = (int)net->convs.size() - 1;
-  int off = 0;
   for (int l = 0; l < 5; ++l) {
-    const int Hl = net->acts[lv[l]].H;
-    net->level_size[l] = Hl; net->level_off[l] = off;
-    off += Hl * Hl * R;
+    net->level_size[l] = net->acts[lv[l]].H;
     const int f = add_conv(net, lv[l], upf, 1, 1);
     const int h = add_conv(net, f, head, 1, 0, -1, 1);
     Op o; o.kind = OP_HEADFIN; o.in = h; o.level = l; net->ops.push_back(o);
   }
-  net->A = off;
-
-  // anchors (utils/box_utils.py:86-101, modules/yolact.py:111-114): float64, rounded once
-  net->anchors.resize((size_t)net->A * 4);
-  const double ars[3] = {1.0, 0.5, 2.0};
-  size_t q = 0;
-  for (int l = 0; l < 5; ++l) {
-    const int size = net->level_size[l];
-    const double scale = (double)(int)((double)S / 544.0 * (double)(24 << l));
-    for (int j = 0; j < size; ++j)
-      for (int i = 0; i < size; ++i)
-        for (int r = 0; r < R; ++r) {
-          const double ar = sqrt(ars[r % 3]);
-          net->anchors[q++] = (float)((i + 0.5) / size);
-          net->anchors[q++] = (float)((j + 0.5) / size);
-          net->anchors[q++] = (float)(scale * ar / S);
-          net->anchors[q++] = (float)(scale / ar / S);
-        }
-  }
+  net->A = level_offsets(net->level_size, cfg.num_ratios, net->level_off);
+  net->anchors = default_anchors(cfg, net->level_size);
 }
 
 // 16-bit modes: merge [1x1 Cin->Cexp + residual + ReLU] followed by [1x1 Cexp->Cout + ReLU] (conv3 of a bottleneck and conv1 of the
@@ -529,22 +499,8 @@ void conv_args(const yb_net* net, const Op& o, int B, ConvArgs* a, void* ext_out
   a->relu = o.relu; a->out_mode = o.out_mode;
   const int Wp = in.H + 2;
   const long long plane_rows = (long long)net->max_batch * Wp * Wp;      // parity planes sit at max-batch strides
-  a->in_rows = plane_rows * in.planes;
-  if (o.stride == 1) {
-    a->ntaps = c.k * c.k;
-    for (int r = 0; r < c.k; ++r)
-      for (int s = 0; s < c.k; ++s) a->tap_shift[r * c.k + s] = c.k == 1 ? 0 : (r - 1) * Wp + (s - 1);
-    a->in_rows = (long long)B * Wp * Wp;
-  } else if (c.k == 1) {
-    a->ntaps = 1; a->tap_shift[0] = 0;
-  } else {
-    a->ntaps = 9;
-    for (int r = 0; r < 3; ++r)
-      for (int s = 0; s < 3; ++s) {
-        const int pr = r == 1 ? 0 : 1, ps = s == 1 ? 0 : 1, dy = r == 0 ? -1 : 0, dx = s == 0 ? -1 : 0;
-        a->tap_shift[r * 3 + s] = (int)((pr * 2 + ps) * plane_rows) + dy * Wp + dx;
-      }
-  }
+  a->in_rows = o.stride == 1 ? (long long)B * Wp * Wp : plane_rows * in.planes;
+  a->ntaps = conv_taps(c.k, o.stride, Wp, plane_rows, a->tap_shift);
 }
 
 }  // namespace
@@ -687,7 +643,7 @@ extern "C" int yb_net_finalize(yb_net* net, int max_batch, int precision) {
       a.in = act_ptr(net, so.aux); a.weight = net->d_stem_w16; a.bias = net->d_stem_b16; a.out = act_ptr(net, so.out);
       a.act_dt = net->act_dt; a.B = max_batch; a.g.H = net->H1; a.g.W = net->H1; a.Cin = 64; a.Cin_pad = 64; a.Cout = 64; a.Cout_pad = 64;
       a.ntaps = 4; a.relu = 1; a.out_mode = 0;
-      for (int dy = 0; dy < 4; ++dy) a.tap_shift[dy] = (dy - 1) * (net->H1 + 2) - 1;
+      stem_taps(net->H1 + 2, a.tap_shift);
       a.in_rows = (long long)max_batch * (net->H1 + 2) * (net->H1 + 2);
       if (!net->stem_wide) a.in_row_stride = 16;                      // rows overlap: row p = pixels p .. p+3 (3 spare pixels exist: pad_rows)
       YB_PROPAGATE(tc_plan_create(a, max_batch, &so.tc));
@@ -1210,7 +1166,7 @@ extern "C" int yb_conv2d(const float* x, int batch, int cin, int h, const float*
   YB_REQUIRE(precision >= 0 && precision <= 2, YB_ERR_INVALID, "yb_conv2d: precision=%d", precision);
   const int dt = precision == YB_PREC_BF16 ? DT_BF16 : (precision == YB_PREC_FP16 ? DT_F16 : DT_F32);
   const size_t esz = dtype_size(dt);
-  const int ho = stride == 2 ? (h - 1) / 2 + 1 : h;
+  const int ho = out_size(h, stride);
   const int planes = stride == 2 ? (k == 3 ? 4 : 1) : 1;
   const int cout_pad = (cout + 15) / 16 * 16, cout_alloc = (cout_pad + 63) / 64 * 64;
   const int k2 = k * k, Ktot = k2 * cin_pad;
@@ -1246,20 +1202,8 @@ extern "C" int yb_conv2d(const float* x, int batch, int cin, int h, const float*
   a.in = stride == 2 ? d_split : d_in; a.weight = d_w; a.bias = d_b; a.residual = d_res; a.out = d_out;
   a.act_dt = dt; a.B = batch; a.g.H = ho; a.g.W = ho; a.Cin = cin; a.Cin_pad = cin_pad; a.Cout = cout; a.Cout_pad = cout; a.relu = relu; a.out_mode = 0;
   YB_REQUIRE(cout % 16 == 0 || !use_tc, YB_ERR_UNSUPPORTED, "yb_conv2d: tc path needs cout %% 16 == 0");
-  const int Wp = ho + 2;
-  if (stride == 1) {
-    a.ntaps = k2;
-    for (int r = 0; r < k; ++r) for (int s = 0; s < k; ++s) a.tap_shift[r * k + s] = k == 1 ? 0 : (r - 1) * Wp + (s - 1);
-    a.in_rows = (long long)out_rows;
-  } else if (k == 1) {
-    a.ntaps = 1; a.tap_shift[0] = 0; a.in_rows = (long long)out_rows;
-  } else {
-    a.ntaps = 9; a.in_rows = (long long)out_rows * 4;
-    for (int r = 0; r < 3; ++r) for (int s = 0; s < 3; ++s) {
-      const int pr = r == 1 ? 0 : 1, ps = s == 1 ? 0 : 1, dy = r == 0 ? -1 : 0, dx = s == 0 ? -1 : 0;
-      a.tap_shift[r * 3 + s] = (int)((pr * 2 + ps) * (long long)out_rows) + dy * Wp + dx;
-    }
-  }
+  a.ntaps = conv_taps(k, stride, ho + 2, (long long)out_rows, a.tap_shift);
+  a.in_rows = (long long)out_rows * planes;
   if (use_tc) {
     YB_REQUIRE(tc_supported(a), YB_ERR_UNSUPPORTED, "yb_conv2d: shape/precision not supported by the wgmma kernel");
     TcPlan* pl = nullptr;

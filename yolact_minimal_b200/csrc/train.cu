@@ -13,9 +13,9 @@
 // The program is built ONCE per engine (fixed batch): every buffer, TMA descriptor and launch closure is created up front, a
 // step replays the two lists.  Parameters are never copied: yb_train_bind stores the caller's device pointers (fp32 master
 // weights and their gradient buffers); each forward re-packs the 16-bit operand copies from them in one batched launch.
+#include "arch.cuh"
 #include "train.cuh"
 
-#include <math.h>
 #include <stdlib.h>
 #include <string.h>
 #include <functional>
@@ -60,7 +60,7 @@ struct ConvRec {                  // one convolution's parameters (possibly used
   bool wgrad_set = false, needs_dgrad_w = true;
   int bias_idx = -1;              // bound-tensor index of the bias parameter (resolved at launch time: bindings come after build)
   int tapslot[9];
-  int plane_slot0[4], plane_ntaps[4];
+  int plane_slot0[4];
 };
 
 typedef std::function<int(cudaStream_t)> Launch;
@@ -69,7 +69,7 @@ typedef std::function<int(cudaStream_t)> Launch;
 
 struct yb_train {
   yb_net_config cfg{};
-  int B = 0, dt = DT_BF16, S = 0, H1 = 0, H2 = 0;
+  int B = 0, dt = DT_BF16, S = 0;
   int A = 0, P = 0, Hs = 0;
   int level_size[5]{}, level_off[5]{};
   std::vector<BoundTensor> bound;
@@ -174,25 +174,16 @@ ConvRec* new_conv(yb_train* t, const std::string& prefix, int Cin, int Cout, int
 
 void conv_tap_layout(ConvRec* c) {
   const int k2 = c->k * c->k;
-  for (int i = 0; i < 4; ++i) { c->plane_slot0[i] = 0; c->plane_ntaps[i] = 0; }
+  for (int i = 0; i < 4; ++i) c->plane_slot0[i] = 0;
   if (c->stride == 1 || c->k == 1) {
     for (int tt = 0; tt < k2; ++tt) c->tapslot[tt] = k2 - 1 - tt;          // reversed taps: dgrad shifts == forward shifts
-    c->plane_ntaps[0] = k2;
-  } else {
-    // 3x3 stride 2: forward tap (r, s) reads parity plane (r != 1, s != 1) at (dy, dx) = (r == 0 ? -1 : 0, s == 0 ? -1 : 0).
-    // dgrad of plane p = conv over dY with that plane's taps at shifts -(dy*Wp + dx), slots ordered by ascending shift.
+  } else {                                                                  // 3x3 stride 2: each plane's taps, in dgrad shift order
     int slot = 0;
     for (int pl = 0; pl < 4; ++pl) {
+      int taps[4];
       c->plane_slot0[pl] = slot;
-      for (int sdy = 0; sdy <= 1; ++sdy)
-        for (int sdx = 0; sdx <= 1; ++sdx)
-          for (int r = 0; r < 3; ++r)
-            for (int s = 0; s < 3; ++s) {
-              const int pr = r == 1 ? 0 : 1, ps = s == 1 ? 0 : 1, dy = r == 0 ? -1 : 0, dx = s == 0 ? -1 : 0;
-              if (pr * 2 + ps != pl || -dy != sdy || -dx != sdx) continue;
-              c->tapslot[r * 3 + s] = slot++;
-            }
-      c->plane_ntaps[pl] = slot - c->plane_slot0[pl];
+      const int n = parity_plane_taps(pl, taps);
+      for (int i = 0; i < n; ++i) c->tapslot[taps[i]] = slot++;
     }
   }
 }
@@ -233,28 +224,10 @@ void add_pack_descs(yb_train* t, ConvRec* c) {
   }
 }
 
-// geometry helpers
-void fill_taps_fwd(const ConvRec* c, int Wp, long long plane_rows, int* ntaps, int* shift) {
-  if (c->stride == 1) {
-    *ntaps = c->k * c->k;
-    for (int r = 0; r < c->k; ++r)
-      for (int s = 0; s < c->k; ++s) shift[r * c->k + s] = c->k == 1 ? 0 : (r - 1) * Wp + (s - 1);
-  } else if (c->k == 1) {
-    *ntaps = 1; shift[0] = 0;
-  } else {
-    *ntaps = 9;
-    for (int r = 0; r < 3; ++r)
-      for (int s = 0; s < 3; ++s) {
-        const int pr = r == 1 ? 0 : 1, ps = s == 1 ? 0 : 1, dy = r == 0 ? -1 : 0, dx = s == 0 ? -1 : 0;
-        shift[r * 3 + s] = (int)((pr * 2 + ps) * plane_rows) + dy * Wp + dx;
-      }
-  }
-}
-
 // ---- forward conv op + its backward ----
 // x: input (haloed, planes == 1); returns y (raw conv output + bias, optional fused ReLU; haloed 16-bit, or dense fp32 [B*Ho*Ho][Cout_pad])
 int op_conv(yb_train* t, TT* x, ConvRec* c, int relu, bool out_dense, const std::string& yname, TT** out, TT* y_given = nullptr) {
-  const int B = t->B, Hin = x->H, Hout = c->stride == 2 ? (Hin - 1) / 2 + 1 : Hin, Wp = Hout + 2;
+  const int B = t->B, Hin = x->H, Hout = out_size(Hin, c->stride), Wp = Hout + 2;
   t->cur_label = "conv " + yname;
   const long long plane_rows = (long long)B * Wp * Wp;
   TT* src = x;
@@ -277,7 +250,7 @@ int op_conv(yb_train* t, TT* x, ConvRec* c, int relu, bool out_dense, const std:
   a.act_dt = t->dt; a.B = B; a.g.H = Hout; a.g.W = Hout;
   a.Cin = c->Cin; a.Cin_pad = c->Cin_pad; a.Cout = out_dense ? c->Cout : c->Cout_pad; a.Cout_pad = c->Cout_pad;
   a.relu = relu; a.out_mode = out_dense ? 1 : 0;
-  fill_taps_fwd(c, Wp, plane_rows, &a.ntaps, a.tap_shift);
+  a.ntaps = conv_taps(c->k, c->stride, Wp, plane_rows, a.tap_shift);
   a.in_rows = src->rows;
   YB_REQUIRE(tc_supported(a), YB_ERR_UNSUPPORTED, "train: conv %s (Cin=%d Cout=%d) not supported by the wgmma kernel", c->wname.c_str(), c->Cin, c->Cout);
   TcPlan* pl = nullptr;
@@ -318,7 +291,7 @@ int op_conv(yb_train* t, TT* x, ConvRec* c, int relu, bool out_dense, const std:
       GemmArgs g; memset(&g, 0, sizeof(g));
       g.a = dyT; g.b = src->data; g.out = c->dWp; g.act_dt = dt; g.M = c->Cout_pad; g.Nper = c->Cin_pad; g.K = (int)rows_y; g.lda = (int)ldT; g.ldb = src->C;
       g.Kb = src->rows; g.accumulate = 1;                           // dWp is zero at the start of a backward pass (cleared by the unpack kernel)
-      fill_taps_fwd(c, Wp, plane_rows, &g.ntaps, g.shift);
+      g.ntaps = conv_taps(c->k, c->stride, Wp, plane_rows, g.shift);
       {  // split-K: a weight gradient has few output tiles and a long K (the pixels); cut K so that ~2 waves of CTAs are busy
         const int bn = c->Cin_pad % 256 == 0 ? 256 : (c->Cin_pad % 128 == 0 ? 128 : 64);
         const int tiles = ((c->Cout_pad + 127) / 128) * g.ntaps * (c->Cin_pad / bn);
@@ -344,8 +317,7 @@ int op_conv(yb_train* t, TT* x, ConvRec* c, int relu, bool out_dense, const std:
         d.in = dy; d.weight = c->wb; d.bias = t->zeros; d.residual = x->grad_set ? x->grad : nullptr; d.out = x->grad;
         d.act_dt = dt; d.B = B; d.g.H = Hout; d.g.W = Hout; d.Cin = Cg; d.Cin_pad = c->CoutT_pad; d.Cout = c->Cin; d.Cout_pad = c->Cin;
         d.relu = 0; d.out_mode = 0; d.in_rows = rows_y;
-        int nt; fill_taps_fwd(c, Wp, plane_rows, &nt, d.tap_shift);
-        d.ntaps = nt;
+        d.ntaps = conv_taps(c->k, c->stride, Wp, plane_rows, d.tap_shift);
         YB_REQUIRE(tc_supported(d), YB_ERR_UNSUPPORTED, "train: dgrad of %s not supported", c->wname.c_str());
         TcPlan* dp = nullptr;
         YB_PROPAGATE(tc_plan_create(d, B, &dp));
@@ -361,22 +333,8 @@ int op_conv(yb_train* t, TT* x, ConvRec* c, int relu, bool out_dense, const std:
           d.bias = t->zeros; d.residual = nullptr; d.out = (char*)dplanes + (size_t)pl_i * plane_rows * c->Cin * 2;
           d.act_dt = dt; d.B = B; d.g.H = Hout; d.g.W = Hout; d.Cin = Cg; d.Cin_pad = c->CoutT_pad; d.Cout = c->Cin; d.Cout_pad = c->Cin;
           d.relu = 0; d.out_mode = 0; d.in_rows = rows_y;
-          d.ntaps = c->plane_ntaps[pl_i];
-          if (c->k == 1) d.tap_shift[0] = 0;
-          else {
-            int q = 0;
-            for (int sdy = 0; sdy <= 1; ++sdy)
-              for (int sdx = 0; sdx <= 1; ++sdx) {
-                // does this plane have a tap with (-dy, -dx) == (sdy, sdx)?
-                bool has = false;
-                for (int r = 0; r < 3 && !has; ++r)
-                  for (int s2 = 0; s2 < 3 && !has; ++s2) {
-                    const int pr = r == 1 ? 0 : 1, ps = s2 == 1 ? 0 : 1, dyy = r == 0 ? -1 : 0, dxx = s2 == 0 ? -1 : 0;
-                    has = (pr * 2 + ps == pl_i) && -dyy == sdy && -dxx == sdx;
-                  }
-                if (has) d.tap_shift[q++] = sdy * Wp + sdx;
-              }
-          }
+          int taps[4];
+          d.ntaps = c->k == 1 ? 1 : parity_plane_taps(pl_i, taps, Wp, d.tap_shift);
           YB_REQUIRE(tc_supported(d), YB_ERR_UNSUPPORTED, "train: stride-2 dgrad of %s not supported", c->wname.c_str());
           TcPlan* dp = nullptr;
           YB_PROPAGATE(tc_plan_create(d, B, &dp));
@@ -605,8 +563,7 @@ int op_merge(yb_train* t, TT* x, const std::string& mname, TT** out) {
 // Swin-T backbone (modules/swin_transformer.py:436-518, as net.cu's depth-0 program): patch embedding, 4 stages of (shifted-)window
 // blocks with stochastic depth, patch merging; couts[1..3] = backbone.norm1..3 (tensors "c3", "c4", "c5")
 int build_swin(yb_train* t, std::vector<ConvRec*>* all, TT** couts) {
-  const int B = t->B, S = t->S, dt = t->dt, Hg = (S + 3) / 4;
-  const int depths[4] = {2, 2, 6, 2}, heads[4] = {3, 6, 12, 24};
+  const int B = t->B, S = t->S, dt = t->dt, Hg = stem_sizes(S).Hg;
   YB_PROPAGATE(dev_alloc(t, (void**)&t->drop_masks, (size_t)B * kSwinBlocks * 2 * 4));
   {
     float* masks = t->drop_masks;
@@ -654,14 +611,14 @@ int build_swin(yb_train* t, std::vector<ConvRec*>* all, TT** couts) {
   int blk = 0;
   for (int st = 0; st < 4; ++st) {
     const int C = 96 << st;
-    for (int b = 0; b < depths[st]; ++b, ++blk) {
+    for (int b = 0; b < kSwinDepths[st]; ++b, ++blk) {
       const std::string p = "backbone.layers." + std::to_string(st) + ".blocks." + std::to_string(b);
       TT *t1, *qkv, *att, *y, *x1, *t2, *h, *g, *y2;
       ConvRec *cq, *cp, *c1, *c2;
       YB_PROPAGATE(op_ln(t, x, p + ".norm1", p + ".norm1", &t1));
       YB_PROPAGATE(swin_linear(t, p + ".attn.qkv", C, 3 * C, true, all, &cq));
       YB_PROPAGATE(op_conv(t, t1, cq, 0, false, p + ".attn.qkv", &qkv));
-      YB_PROPAGATE(op_attn(t, qkv, cq, p, heads[st], (b % 2) ? 3 : 0, &att));
+      YB_PROPAGATE(op_attn(t, qkv, cq, p, kSwinHeads[st], (b % 2) ? 3 : 0, &att));
       YB_PROPAGATE(swin_linear(t, p + ".attn.proj", C, C, true, all, &cp));
       YB_PROPAGATE(op_conv(t, att, cp, 0, false, p + ".attn.proj", &y));
       YB_PROPAGATE(op_drop_residual(t, x, y, blk, 0, p + ".x1", &x1));
@@ -690,7 +647,7 @@ int build_swin(yb_train* t, std::vector<ConvRec*>* all, TT** couts) {
 int build(yb_train* t) {
   const yb_net_config& cfg = t->cfg;
   const int B = t->B, S = cfg.img_size, dt = t->dt;
-  t->S = S; t->H1 = (S - 1) / 2 + 1; t->H2 = (t->H1 - 1) / 2 + 1;
+  t->S = S;
   YB_PROPAGATE(dev_alloc(t, (void**)&t->zeros, 4096 * 4));
   YB_PROPAGATE(dev_alloc(t, (void**)&t->d_img, (size_t)B * 3 * S * S * 4));
   TT* couts[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -700,7 +657,8 @@ int build(yb_train* t) {
   } else {
 
   // ---------------- stem: space-to-depth image -> 4-tap K=64 conv -> BN -> ReLU -> max-pool ----------------
-  const int H1 = t->H1, Wp1 = H1 + 2;
+  const StemSizes ss = stem_sizes(S);
+  const int H1 = ss.H1, H2 = ss.H2, Wp1 = H1 + 2;
   t->add_bound("backbone.conv1.weight", 64 * 3 * 7 * 7, 0);
   TT* s2d = new_tensor(t, "stem.s2d", 64, H1);            // 4 pixels x 16 channels per row (materialised: rows are self-contained)
   YB_PROPAGATE(alloc_data(t, s2d));
@@ -717,7 +675,7 @@ int build(yb_train* t) {
     ConvArgs a; memset(&a, 0, sizeof(a));
     a.in = s2d->data; a.weight = w16; a.bias = t->zeros; a.out = sy->data; a.act_dt = dt; a.B = B; a.g.H = H1; a.g.W = H1;
     a.Cin = 64; a.Cin_pad = 64; a.Cout = 64; a.Cout_pad = 64; a.ntaps = 4; a.relu = 0; a.out_mode = 0;
-    for (int dy = 0; dy < 4; ++dy) a.tap_shift[dy] = (dy - 1) * Wp1 - 1;
+    stem_taps(Wp1, a.tap_shift);
     a.in_rows = s2d->rows;
     TcPlan* pl = nullptr;
     YB_PROPAGATE(tc_plan_create(a, B, &pl));
@@ -736,7 +694,7 @@ int build(yb_train* t) {
       GemmArgs g; memset(&g, 0, sizeof(g));
       g.a = dyT; g.b = s2dd; g.out = dW16; g.act_dt = dt; g.M = 64; g.Nper = 64; g.K = (int)rows; g.lda = (int)ldT; g.ldb = 64; g.Kb = rows; g.ntaps = 4;
       g.accumulate = 1; g.splits = 74;                              // 4 output tiles, K = every pixel of the batch: split-K
-      for (int dy_ = 0; dy_ < 4; ++dy_) g.shift[dy_] = (dy_ - 1) * Wp1 - 1;        // out [64][dy*64 + dx*16 + e]: the packed stem layout
+      stem_taps(Wp1, g.shift);                                      // out [64][dy*64 + dx*16 + e]: the packed stem layout
       TcPlan* gp = nullptr;
       YB_PROPAGATE(tc_plan_create_gemm(g, &gp));
       t->plans.push_back(gp);
@@ -747,10 +705,10 @@ int build(yb_train* t) {
   }
   TT* sz = nullptr;
   YB_PROPAGATE(op_bn(t, sy, "backbone.bn1", 1, nullptr, "stem.z", &sz));
-  TT* x = new_tensor(t, "pool", 64, t->H2);
+  TT* x = new_tensor(t, "pool", 64, H2);
   YB_PROPAGATE(alloc_data(t, x));
   {
-    void* in = sz->data; void* out = x->data; const int H2 = t->H2;
+    void* in = sz->data; void* out = x->data;
     FWD_PUSH([=](cudaStream_t s) { return launch_maxpool(in, out, dt, B, 64, H1, H2, s); });
     TT* xx = x;
     t->bwd_builders.push_back([=]() -> int {
@@ -764,8 +722,7 @@ int build(yb_train* t) {
   }
 
   // ---------------- bottleneck stages (modules/resnet.py:46-98) ----------------
-  const int nblk50[4] = {3, 4, 6, 3}, nblk101[4] = {3, 4, 23, 3};
-  const int* nblk = cfg.depth == 50 ? nblk50 : nblk101;
+  const int* nblk = resnet_blocks(cfg.depth);
   int inpl = 64;
   for (int st = 0; st < 4; ++st) {
     const int planes = 64 << st;
@@ -878,12 +835,11 @@ int build(yb_train* t) {
   std::unique_ptr<ConvRec> hu(new ConvRec());
   ConvRec* hc = hu.get();
   t->convs.push_back(std::move(hu));
-  hc->Cin = 256; hc->Cin_pad = 256; hc->k = 3; hc->stride = 1; hc->Cout = R * (NC + 4 + K); hc->Cout_pad = (hc->Cout + 15) / 16 * 16;
+  const HeadLayout hl = head_layout(cfg);
+  hc->Cin = 256; hc->Cin_pad = 256; hc->k = 3; hc->stride = 1; hc->Cout = hl.Cout; hc->Cout_pad = hl.Cout_pad;
   hc->CoutT_pad = (hc->Cout_pad + 63) / 64 * 64;
-  hc->cat = {"prediction_layers.conf_layer", "prediction_layers.bbox_layer", "prediction_layers.coef_layer.0"};
-  t->add_bound("prediction_layers.bbox_layer.weight", (int64_t)R * 4 * 256 * 9, 0); t->add_bound("prediction_layers.bbox_layer.bias", R * 4, 0);
-  t->add_bound("prediction_layers.conf_layer.weight", (int64_t)R * NC * 256 * 9, 0); t->add_bound("prediction_layers.conf_layer.bias", R * NC, 0);
-  t->add_bound("prediction_layers.coef_layer.0.weight", (int64_t)R * K * 256 * 9, 0); t->add_bound("prediction_layers.coef_layer.0.bias", R * K, 0);
+  hc->cat = hl.cat;
+  for (const auto& p : hl.params) t->add_bound(p.first, p.second, 0);
   YB_PROPAGATE(alloc_conv(t, hc, true));
   YB_PROPAGATE(dev_alloc(t, (void**)&hc->bias_cat, (size_t)hc->Cout_pad * 4));
   hc->bias = hc->bias_cat;
@@ -898,9 +854,8 @@ int build(yb_train* t) {
       row += cnt;
     }
   }
-  int off = 0;
-  for (int l = 0; l < 5; ++l) { t->level_size[l] = lv[l]->H; t->level_off[l] = off; off += lv[l]->H * lv[l]->H * R; }
-  t->A = off;
+  for (int l = 0; l < 5; ++l) t->level_size[l] = lv[l]->H;
+  t->A = level_offsets(t->level_size, R, t->level_off);
   const size_t BA = (size_t)B * t->A;
   YB_PROPAGATE(dev_alloc(t, (void**)&t->cls, BA * NC * 4)); YB_PROPAGATE(dev_alloc(t, (void**)&t->box, BA * 16)); YB_PROPAGATE(dev_alloc(t, (void**)&t->coef, BA * K * 4));
   YB_PROPAGATE(dev_alloc(t, (void**)&t->g_cls, BA * NC * 4)); YB_PROPAGATE(dev_alloc(t, (void**)&t->g_box, BA * 16)); YB_PROPAGATE(dev_alloc(t, (void**)&t->g_coef, BA * K * 4));
@@ -946,23 +901,7 @@ int build(yb_train* t) {
 
   // the builders above were registered in forward order EXCEPT that a dense output's gradient scatter must run BEFORE its conv's
   // backward: they were registered after the conv (so they run first in the reversed order) -- as required.
-  // ---------------- anchors ----------------
-  t->anchors.resize((size_t)t->A * 4);
-  {
-    const double ars[3] = {1.0, 0.5, 2.0};
-    size_t qn = 0;
-    for (int l = 0; l < 5; ++l) {
-      const int size = t->level_size[l];
-      const double scale = (double)(int)((double)S / 544.0 * (double)(24 << l));
-      for (int j = 0; j < size; ++j)
-        for (int i = 0; i < size; ++i)
-          for (int r = 0; r < R; ++r) {
-            const double ar = sqrt(ars[r % 3]);
-            t->anchors[qn++] = (float)((i + 0.5) / size); t->anchors[qn++] = (float)((j + 0.5) / size);
-            t->anchors[qn++] = (float)(scale * ar / S); t->anchors[qn++] = (float)(scale / ar / S);
-          }
-    }
-  }
+  t->anchors = default_anchors(cfg, t->level_size);
   YB_PROPAGATE(dev_alloc(t, (void**)&t->d_anchors, t->anchors.size() * 4));
   YB_CHECK_CUDA(cudaMemcpy(t->d_anchors, t->anchors.data(), t->anchors.size() * 4, cudaMemcpyHostToDevice));
   YB_PROPAGATE(dev_alloc(t, (void**)&t->d_losses_scratch, 16));
